@@ -1,0 +1,106 @@
+"""The pipelined flash-attention loop against the serial one (VX_FA_V1=1): same key order, same accumulation order, same
+rounding points, so the outputs are compared bit for bit (GPU)."""
+import os
+
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(scope="module")
+def ops():
+    from vexpress_b200 import _ffi, ops
+    _ffi.require_sm90()
+    return ops
+
+
+@pytest.fixture
+def serial_loop():
+    """Context-free switch: serial_loop(True) routes every head dim to the serial loop until serial_loop(False)."""
+    from vexpress_b200 import _ffi
+    before = os.environ.get("VX_FA_V1")
+
+    def switch(on):
+        if on:
+            os.environ["VX_FA_V1"] = "1"
+        else:
+            os.environ.pop("VX_FA_V1", None)
+        _ffi.lib().vx_flash_reload_env()
+
+    yield switch
+    if before is None:
+        os.environ.pop("VX_FA_V1", None)
+    else:
+        os.environ["VX_FA_V1"] = before
+    _ffi.lib().vx_flash_reload_env()
+
+
+def _inputs(B, N, heads, hd, kv_div, Nk):
+    g = torch.Generator(device="cuda").manual_seed(B * N + hd + Nk)
+    C = heads * hd
+    Bkv = (B + kv_div - 1) // kv_div
+    q = torch.randn(B * N, C, device="cuda", generator=g).bfloat16()
+    kv = (1.5 * torch.randn(Bkv * Nk, 2 * C, device="cuda", generator=g)).bfloat16()
+    return q, kv[:, :C], kv[:, C:]
+
+
+# (3, 384, 8, 40, 3, 336): Nk = 5 * 64 + 16, the key tail is masked under two consumer warpgroups;
+# (2, 192, ..) / (2, 80, ..): Nq is not a multiple of 128 / 64, tiles run into the next frame and past the last row
+@pytest.mark.parametrize("B,N,heads,hd,kv_div,Nk", [(4, 4096, 8, 40, 1, 4096), (4, 1024, 8, 80, 1, 1024),
+                                                    (4, 256, 8, 160, 1, 256), (4, 64, 8, 160, 1, 64),
+                                                    (4, 1024, 8, 80, 2, 512), (3, 384, 8, 40, 3, 336),
+                                                    (2, 192, 8, 40, 1, 192), (2, 80, 8, 40, 1, 80),
+                                                    # one consumer warpgroup (Nq <= 64), one step (T = 1), fewer steps than stages
+                                                    (4, 64, 8, 40, 1, 64), (2, 256, 8, 40, 2, 128), (2, 128, 4, 56, 1, 192),
+                                                    (3, 320, 8, 8, 1, 320), (2, 1024, 8, 48, 1, 1024)])
+def test_pipelined_loop_equals_serial_loop(ops, serial_loop, B, N, heads, hd, kv_div, Nk):
+    q, k, v = _inputs(B, N, heads, hd, kv_div, Nk)
+    serial_loop(True)
+    ref = ops.flash_attention(q, k, v, heads, N, Nk, kv_div)
+    serial_loop(False)
+    out = ops.flash_attention(q, k, v, heads, N, Nk, kv_div)
+    torch.cuda.synchronize()
+    assert not torch.isnan(out.float()).any()
+    assert torch.equal(out, ref), f"max abs diff {(out.float() - ref.float()).abs().max().item():.3e}"
+
+
+def test_reference_attention_call_pattern(ops, serial_loop):
+    """attn1_5 of the UNet: the conditional half of the frames attends to one bank per window (kv_div = f) and writes into
+    the second half of a shared buffer; the first half must stay as it was."""
+    f, HW, heads, hd = 4, 1024, 8, 40
+    C = heads * hd
+    g = torch.Generator(device="cuda").manual_seed(15)
+    q = torch.randn(2 * f * HW, C, device="cuda", generator=g).bfloat16()
+    bank = torch.randn(HW, 2 * C, device="cuda", generator=g).bfloat16()
+    outs = []
+    for serial in (True, False):
+        serial_loop(serial)
+        a = torch.full((2 * f * HW, C), 7.0, device="cuda", dtype=torch.bfloat16)
+        ops.flash_attention(q[f * HW:], bank[:, :C], bank[:, C:], heads, HW, HW, kv_div=f, out=a[f * HW:])
+        torch.cuda.synchronize()
+        assert torch.all(a[:f * HW] == 7.0)
+        outs.append(a[f * HW:].clone())
+    assert torch.equal(outs[0], outs[1])
+    qf = q[f * HW:].float().view(f, HW, heads, hd).transpose(1, 2)
+    kf, vf = (t.float().view(1, HW, heads, hd).transpose(1, 2).expand(f, -1, -1, -1) for t in (bank[:, :C], bank[:, C:]))
+    ref = torch.nn.functional.scaled_dot_product_attention(qf, kf, vf).transpose(1, 2).reshape(f * HW, C)
+    rel = ((outs[1].float() - ref).norm() / ref.norm()).item()
+    assert rel < 4e-3, rel
+
+
+@pytest.mark.parametrize("B,N,heads,hd", [(2, 4096, 8, 40), (8, 1024, 8, 80)])
+def test_pipelined_loop_is_deterministic(ops, B, N, heads, hd):
+    """A ring or register hazard between in-flight MMAs shows up as run-to-run differences first."""
+    g = torch.Generator(device="cuda").manual_seed(B * N + hd)
+    C = heads * hd
+    qkv = torch.randn(B * N, 3 * C, device="cuda", generator=g).bfloat16()
+    first = None
+    for i in range(12):
+        out = ops.flash_attention(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], heads, N, N)
+        if i % 2 == 0:
+            torch.empty(1 << 24, device="cuda").normal_()
+        if first is None:
+            first = out.clone()
+        else:
+            assert torch.equal(out, first), f"run {i} differs from run 0 by {(out.float() - first.float()).abs().max().item():.3e}"

@@ -7,7 +7,7 @@
 // of the window, kv_div = f; :202-219) -- both diffusers AttnProcessor2_0 / F.scaled_dot_product_attention
 // without mask (SURVEY.md Appendix B.2).
 //
-// One CTA = one warpgroup = 64 query rows of one (frame, head); several CTAs share an SM.  Per 64-key step:
+// Per 64-key step, for the 64 query rows of one warpgroup:
 //   TMA   : K_j, V_j tiles -> smem ring (3-D view (8, rows, C/8) of the [rows, C] token matrix, so a head slice
 //           lands as [hd/8][rows][8] = the no-swizzle core-matrix layout; hd = 40 is zero-padded to 48 in smem
 //           only, never in HBM)
@@ -16,6 +16,14 @@
 //           fragment of the next MMA (the accumulator layout of m64n16 is the A layout of m64k16)
 //   wgmma : O += P_j V_j  (A = P from registers, B = V tile MN-major from shared memory)
 // Epilogue: O / l -> bf16 -> out[row, h*hd : (h+1)*hd].
+//
+// Two main loops compute this, with the same key order, the same accumulation order per row and the same rounding
+// points (P -> bf16, O in fp32, O / l -> bf16), so their outputs are bit-identical:
+//   flash_attn_pipe_kernel  : one producer warp + NCONS consumer warpgroups (64 NCONS query rows per CTA) around a
+//                             full / empty mbarrier ring; each warpgroup issues S_{j+1} and O += P_j V_j together and
+//                             runs the softmax of S_{j+1} under the latter.  Serves hd <= kFaPipeMaxHd.
+//   flash_attn_wgmma_kernel : one CTA = one warpgroup = 64 query rows, each step a serial chain.  Serves the wider
+//                             heads, and every head dim under VX_FA_V1=1 (the A/B reference).
 #include "vx_host.h"
 #include "vx_ptx.cuh"
 
@@ -159,16 +167,227 @@ flash_attn_wgmma_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_c
   }
 }
 
-template <int HDP>
-static cudaError_t launch_fa(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& mQ, const CUtensorMap& mK,
-                             const CUtensorMap& mV, const FaArgs& a) {
+// ---------------------------------------------------------------------------------------------------------------------
+// Pipelined loop.  Warpgroup 0 is the producer: its warp 0 issues every TMA, and the warpgroup hands its registers to the
+// consumers.  Warpgroups 1 .. NCONS are the consumers, 64 query rows each, sharing every K / V stage.
+//
+// Ring: kv_full[s] (one arrival + transaction bytes) completes when K_j and V_j have landed in stage s = j % stages;
+// kv_empty[s] (lane 0 of every consumer warp = 4 NCONS arrivals) completes when every warp's O += P_j V_j has completed.
+// For use n = j / stages of a stage the consumers wait for kv_full parity n & 1, and the producer refills for use n >= 1
+// behind kv_empty parity (n - 1) & 1.  Neither side gets two phases ahead: fill n + 1 needs release n, which needs fill n.
+// A warpgroup whose rows all lie past Nq still consumes and releases every stage; only its stores are suppressed.
+//
+// MMA schedule of a consumer warpgroup, commit groups in issue order:
+//   prologue     [S_0]                         wait<0>   softmax(S_0) -> l, P_0
+//   j < T - 1    [S_{j+1}]  [O += P_j V_j]     wait<1>   S_{j+1} complete, O += P_j V_j may still run:
+//                                                        softmax(S_{j+1}) in place -> alpha, l   (under the P V MMA)
+//                                              wait<0>   O += P_j V_j complete: release stage j, O *= alpha, pack P_{j+1}
+//   j = T - 1    [O += P_j V_j]                wait<0>   release stage j
+// No MMA is in flight when S_{j+1} issues (the previous iteration ended in wait<0>), so it is never queued behind an
+// incomplete MMA on the same registers.  P_j (register A operand) and O are untouched between the issue of O += P_j V_j
+// and its wait<0>; S is untouched between the issue of S_{j+1} and wait<1>.  wgmma_fence_regs behind each wait keeps the
+// compiler from moving those accesses up, the wgmma_fence in front of each issue orders the thread's own register
+// writes (P, O *= alpha) before the MMAs.
+//
+// The arithmetic is that of flash_attn_wgmma_kernel, operation for operation, spelled with the non-contracting intrinsics
+// (there the compiler contracts l * alpha + (e0 + e1) of the first pair into one FMA; here that is written out).  Two
+// deliberate differences, neither visible in a result: exponentials are the bare ex2.approx.ftz (identical for every value
+// >= 2^-126; smaller ones, which vanish against l >= 1 and O in fp32, flush to zero), and O += P V runs at N = hd rather
+// than the padded width (m64n40k16 for hd 40), so V needs no padding chunk.
+constexpr int kFaPipeMaxHd = 56;   // hd 64 no longer fits the 104 registers a consumer gets with two CTAs per SM
+constexpr int kFaPipeStages = 4;
+
+template <int HD, int NCONS>
+__global__ void __launch_bounds__(128 * (NCONS + 1), 2)
+flash_attn_pipe_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                       const __grid_constant__ CUtensorMap mapV, const FaArgs p) {
+  constexpr int HDP = (HD + 15) / 16 * 16;   // Q / K tile width: the K dimension of S = Q K^T in steps of 16
+  constexpr int kTile = kFaRows * HDP * 2;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+  uint8_t* sQ = smem;                         // NCONS x kTile, one tile per consumer warpgroup
+  uint8_t* sK = sQ + NCONS * kTile;           // stages x kTile
+  uint8_t* sV = sK + p.stages * kTile;        // stages x kTile
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(sV + p.stages * kTile);
+  uint64_t* kv_full = q_full + 1;             // [stages]
+  uint64_t* kv_empty = kv_full + p.stages;    // [stages]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q_tile = blockIdx.x, head = blockIdx.y, bq = blockIdx.z;
+  const int T = (p.Nk + kFaRows - 1) / kFaRows;
+  if (HDP > HD) {
+    // the padding chunk of Q / K must read as exact zeros; TMA only ever writes chunks < hd / 8
+    uint4* z = reinterpret_cast<uint4*>(sQ);
+    for (int i = threadIdx.x; i < (NCONS + 2 * p.stages) * kTile / 16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
+  }
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(&kv_full[s], 1);
+      mbar_init(&kv_empty[s], 4 * NCONS);
+    }
+    fence_barrier_init();
+  }
+  fence_proxy_async_smem();  // generic-proxy zero fill visible to TMA / tensor core (async proxy)
+  __syncthreads();
+  pdl_wait();   // shared-memory fill and barrier init overlapped the previous grid's tail
+
+  const int col_chunk = head * HD / 8;
+  if (warp < 4) {
+    // ------------------------------------------------------------------ producer (one lane)
+    if (NCONS == 2) setmaxnreg_dec<24>();   // 384 threads launch with 80 registers (two CTAs per SM): 24 + 2 x 104 <= 240
+    if (warp == 0 && lane == 0) {
+      tma_prefetch_desc(&mapQ);
+      tma_prefetch_desc(&mapK);
+      tma_prefetch_desc(&mapV);
+      mbar_expect_tx(q_full, NCONS * kFaRows * HD * 2);
+      for (int w = 0; w < NCONS; ++w)
+        tma_load_3d(sQ + w * kTile, &mapQ, q_full, 0, bq * p.Nq + (q_tile * NCONS + w) * kFaRows, col_chunk);
+      const int kv_row0 = (bq / p.kv_div) * p.Nk;
+      int st = 0;
+      uint32_t phase = 0;
+      for (int j = 0; j < T; ++j) {
+        if (j >= p.stages) mbar_wait(&kv_empty[st], phase ^ 1);
+        mbar_expect_tx(&kv_full[st], 2 * kFaRows * HD * 2);
+        tma_load_3d(sK + st * kTile, &mapK, &kv_full[st], 0, kv_row0 + j * kFaRows, col_chunk);
+        tma_load_3d(sV + st * kTile, &mapV, &kv_full[st], 0, kv_row0 + j * kFaRows, col_chunk);
+        if (++st == p.stages) {
+          st = 0;
+          phase ^= 1;
+        }
+      }
+    }
+    return;
+  }
+  // -------------------------------------------------------------------- consumers
+  if (NCONS == 2) setmaxnreg_inc<104>();
+  const int wg = (warp >> 2) - 1;
+  // Q / K: K-major, no swizzle: LBO = 64 rows x 16 B between the 8-wide head-dim chunks, SBO = 128 B between 8-row
+  // groups; +2 chunks (+2048 B = +128 in the address field) per 16 head dims.
+  // V: MN-major (head dim contiguous): LBO = 128 B between 8-key groups, SBO = 64 x 16 B between 8-wide head-dim chunks;
+  // +256 B (= +16) per 16 keys.
+  const uint64_t dq = make_smem_desc(smem_u32(sQ + wg * kTile), kFaRows * 16, 128, SWZ_NONE);
+  const float c = p.scale_log2;
+  const int cq = (lane & 3) * 2;
+  float o[HD / 2], s[32];
+  uint32_t pa[4][4];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, alpha[2];
+
+  auto issue_s = [&](int st) {   // S = Q K^T against stage st, one commit group
+    const uint64_t dk = make_smem_desc(smem_u32(sK + st * kTile), kFaRows * 16, 128, SWZ_NONE);
+#pragma unroll
+    for (int k = 0; k < HDP / 16; ++k) Wgmma<64>::ss<0, 0>(s, dq + (uint64_t)(k * 128), dk + (uint64_t)(k * 128), k);
+    wgmma_commit();
+  };
+  auto softmax = [&](int j) {    // scores of step j in s -> alpha, m_run, l; s becomes the unrounded P
+    if ((j + 1) * kFaRows > p.Nk) {   // keys past Nk (the last, partial step) do not exist
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (j * kFaRows + (i >> 2) * 8 + cq + (i & 1) >= p.Nk) s[i] = -INFINITY;
+    }
+    float mc[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int g = 0; g < 8; ++g) mx = fmaxf(mx, fmaxf(s[4 * g + 2 * h], s[4 * g + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx);   // finite: every step holds at least one real key
+      alpha[h] = ex2_ftz(__fmul_rn(__fsub_rn(m_run[h], m_new), c));   // first step: ex2(-inf) = 0
+      m_run[h] = m_new;
+      mc[h] = __fmul_rn(m_new, c);
+    }
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int h = (i >> 1) & 1;
+      s[i] = ex2_ftz(__fmaf_rn(s[i], c, -mc[h]));
+      s[i + 1] = ex2_ftz(__fmaf_rn(s[i + 1], c, -mc[h]));
+      const float e = __fadd_rn(s[i], s[i + 1]);
+      l[h] = i < 4 ? __fmaf_rn(l[h], alpha[h], e) : __fadd_rn(l[h], e);
+    }
+  };
+  auto pack = [&]() {            // P -> bf16, straight into the A fragments of O += P V
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) pa[i >> 3][(i >> 1) & 3] = pack_bf16(s[i], s[i + 1]);
+  };
+
+  mbar_wait(q_full, 0);
+  mbar_wait(&kv_full[0], 0);
+  wgmma_fence();
+  issue_s(0);
+  wgmma_wait<0>();
+  wgmma_fence_regs(s);
+  softmax(0);
+  pack();
+  auto issue_pv = [&](int st) {  // O += P V against stage st, one commit group
+    const uint64_t dv = make_smem_desc(smem_u32(sV + st * kTile), 128, kFaRows * 16, SWZ_NONE);
+#pragma unroll
+    for (int k = 0; k < kFaRows / 16; ++k) Wgmma<HD>::template rs<1>(o, pa[k], dv + (uint64_t)(k * 16), 1);
+    wgmma_commit();
+  };
+  auto pv_done = [&](int st) {   // behind wait<0>: O and P are the thread's again, the stage goes back to the producer
+    wgmma_fence_regs(o);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_fence_regs(pa[k]);
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
+  };
+  int st = 0;
+  uint32_t phase = 0;
+  for (int j = 0; j + 1 < T; ++j) {
+    int st1 = st + 1;
+    uint32_t phase1 = phase;
+    if (st1 == p.stages) {
+      st1 = 0;
+      phase1 ^= 1;
+    }
+    mbar_wait(&kv_full[st1], phase1);
+    wgmma_fence();
+    issue_s(st1);
+    issue_pv(st);
+    wgmma_wait<1>();
+    wgmma_fence_regs(s);
+    softmax(j + 1);
+    wgmma_wait<0>();
+    pv_done(st);
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) o[i] = __fmul_rn(o[i], alpha[(i >> 1) & 1]);
+    pack();
+    st = st1;
+    phase = phase1;
+  }
+  wgmma_fence();
+  issue_pv(st);   // the last step has no successor to overlap
+  wgmma_wait<0>();
+  pv_done(st);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float lt = l[h];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+    const float inv = 1.f / lt;
+    const int qrow = (q_tile * NCONS + wg) * kFaRows + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    if (qrow < p.Nq) {   // per row: a tile may run past the frame, into the next frame's rows
+      __nv_bfloat16* op = p.out + ((long long)bq * p.Nq + qrow) * p.ldo + head * HD;
+#pragma unroll
+      for (int g = 0; g < HD / 8; ++g)
+        *reinterpret_cast<uint32_t*>(op + g * 8 + cq) = pack_bf16(o[4 * g + 2 * h] * inv, o[4 * g + 2 * h + 1] * inv);
+    }
+  }
+}
+
+template <auto Kernel>
+static cudaError_t launch_fa(dim3 grid, int threads, size_t smem, cudaStream_t st, const CUtensorMap& mQ,
+                             const CUtensorMap& mK, const CUtensorMap& mV, const FaArgs& a) {
   static bool configured = false;
   if (!configured) {
-    const cudaError_t e = cudaFuncSetAttribute(flash_attn_wgmma_kernel<HDP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  return launch_k(flash_attn_wgmma_kernel<HDP>, grid, dim3(kFaThreads), smem, st, mQ, mK, mV, a);
+  return launch_k(Kernel, grid, dim3(threads), smem, st, mQ, mK, mV, a);
 }
 
 // Fallback for key counts the tensor-core tiling cannot express (Nk < 16 or Nk % 16 != 0, e.g. the 2x2 / 12x12
@@ -234,8 +453,13 @@ __global__ void __launch_bounds__(128) generic_attn_kernel(const GaArgs p) {
 
 using namespace vx;
 
-// The kernel has no bring-up switches; the hook is kept so that tools which re-read them keep linking.
-extern "C" void vx_flash_reload_env() {}
+// VX_FA_V1: every head dim on flash_attn_wgmma_kernel (A/B switch, read once; the tools and tests that time or compare the
+// two loops in one process re-read it through vx_flash_reload_env).
+static bool& fa_v1() {
+  static bool v = getenv("VX_FA_V1") != nullptr;
+  return v;
+}
+extern "C" void vx_flash_reload_env() { fa_v1() = getenv("VX_FA_V1") != nullptr; }
 
 // q: [Bq*Nq, ldq], k/v: [Bkv*Nk, ldk] / [.., ldv] (bf16, heads*hd columns used), out: [Bq*Nq, ldo].
 // kv batch of query batch b is b / kv_div.
@@ -255,9 +479,12 @@ extern "C" int vx_flash_attention(const void* q, long long ldq, const void* k, l
     return 0;
   }
   const int hdp = (hd + 15) / 16 * 16;
-  // K / V ring depth: two stages for the wide heads keep two CTAs per SM resident, three otherwise
-  const int stages = hdp > 96 ? 2 : 3;
-  const size_t smem = (size_t)(1 + 2 * stages) * kFaRows * hdp * 2 + 128 + 128;
+  const bool pipe = hd <= kFaPipeMaxHd && !fa_v1();
+  // query rows per CTA: two consumer warpgroups, one where a single 64-row tile covers the frame
+  const int ncons = pipe && Nq > kFaRows ? 2 : 1;
+  // K / V ring depth of the serial loop: two stages for the wide heads keep two CTAs per SM resident, three otherwise
+  const int stages = pipe ? kFaPipeStages : hdp > 96 ? 2 : 3;
+  const size_t smem = (size_t)(ncons + 2 * stages) * kFaRows * hdp * 2 + 128 + 128;
   CUtensorMap mQ, mK, mV;
   const void* ptrs[3] = {q, k, v};
   const long long lds[3] = {ldq, ldk, ldv};
@@ -273,10 +500,27 @@ extern "C" int vx_flash_attention(const void* q, long long ldq, const void* k, l
   a.Nq = Nq; a.Nk = Nk; a.hd = hd; a.kv_div = kv_div; a.stages = stages;
   a.scale_log2 = 1.4426950408889634f / sqrtf((float)hd);
   a.out = (__nv_bfloat16*)out; a.ldo = ldo;
-  const dim3 grid((Nq + kFaRows - 1) / kFaRows, heads, Bq);
+  const dim3 grid((Nq + ncons * kFaRows - 1) / (ncons * kFaRows), heads, Bq);
+  if (pipe) {
+    const cudaStream_t cs = (cudaStream_t)stream;
+    cudaError_t e;
+    switch (hd) {
+#define VX_FA_CASE(H)                                                                                       \
+    case H:                                                                                                 \
+      if (ncons == 2) e = launch_fa<flash_attn_pipe_kernel<H, 2>>(grid, 384, smem, cs, mQ, mK, mV, a);         \
+      else e = launch_fa<flash_attn_pipe_kernel<H, 1>>(grid, 256, smem, cs, mQ, mK, mV, a);                    \
+      break;
+      VX_FA_CASE(8) VX_FA_CASE(16) VX_FA_CASE(24) VX_FA_CASE(32) VX_FA_CASE(40) VX_FA_CASE(48) VX_FA_CASE(56)
+#undef VX_FA_CASE
+      default: return fail("vx_flash_attention: hd=%d unsupported", hd);
+    }
+    VX_CHECK_CUDA(e);
+    VX_CHECK_CUDA(cudaGetLastError());
+    return 0;
+  }
   switch (hdp) {
 #define VX_FA_CASE(H) \
-    case H: VX_CHECK_CUDA(launch_fa<H>(grid, smem, (cudaStream_t)stream, mQ, mK, mV, a)); break;
+    case H: VX_CHECK_CUDA(launch_fa<flash_attn_wgmma_kernel<H>>(grid, kFaThreads, smem, (cudaStream_t)stream, mQ, mK, mV, a)); break;
     VX_FA_CASE(16) VX_FA_CASE(32) VX_FA_CASE(48) VX_FA_CASE(64) VX_FA_CASE(80) VX_FA_CASE(96) VX_FA_CASE(112) VX_FA_CASE(128)
     VX_FA_CASE(144) VX_FA_CASE(160) VX_FA_CASE(176) VX_FA_CASE(192) VX_FA_CASE(208) VX_FA_CASE(224) VX_FA_CASE(240)
     VX_FA_CASE(256)

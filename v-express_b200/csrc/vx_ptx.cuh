@@ -107,6 +107,11 @@ __device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+template <int N>
+__device__ __forceinline__ void wgmma_fence_regs(uint32_t (&a)[N]) {   // likewise for a register A fragment
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
@@ -132,6 +137,13 @@ __host__ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, 
 }
 
 // ---------------------------------------------------------------- small numeric helpers
+// 2^x on the MUFU pipe, one instruction: equal to exp2f wherever the result is >= 2^-126, zero below (exp2f spends three
+// more instructions per call on those denormal results)
+__device__ __forceinline__ float ex2_ftz(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&v);
