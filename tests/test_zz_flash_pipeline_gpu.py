@@ -36,10 +36,18 @@ def serial_loop():
     _ffi.lib().vx_flash_reload_env()
 
 
-def _inputs(B, N, heads, hd, kv_div, Nk):
+def _inputs(B, N, heads, hd, kv_div, Nk, family="flat"):
+    """family 'flat': today's N(0, 1) queries and N(0, 1.5^2) keys / values; any other family of
+    test_attention_bounds_gpu.family_inputs ('peaked', 'rising', 'tail' take the exponentials below 2^-126, where the
+    pipelined loop's ex2.approx.ftz and the serial loop's exp2f could part), K / V as column halves of one tensor."""
     g = torch.Generator(device="cuda").manual_seed(B * N + hd + Nk)
     C = heads * hd
     Bkv = (B + kv_div - 1) // kv_div
+    if family != "flat":
+        from test_attention_bounds_gpu import family_inputs
+        q, k, v = family_inputs(family, g, B, N, Bkv, Nk, heads, hd)
+        kv = torch.cat([k, v], 1)
+        return q, kv[:, :C], kv[:, C:]
     q = torch.randn(B * N, C, device="cuda", generator=g).bfloat16()
     kv = (1.5 * torch.randn(Bkv * Nk, 2 * C, device="cuda", generator=g)).bfloat16()
     return q, kv[:, :C], kv[:, C:]
@@ -47,15 +55,19 @@ def _inputs(B, N, heads, hd, kv_div, Nk):
 
 # (3, 384, 8, 40, 3, 336): Nk = 5 * 64 + 16, the key tail is masked under two consumer warpgroups;
 # (2, 192, ..) / (2, 80, ..): Nq is not a multiple of 128 / 64, tiles run into the next frame and past the last row
-@pytest.mark.parametrize("B,N,heads,hd,kv_div,Nk", [(4, 4096, 8, 40, 1, 4096), (4, 1024, 8, 80, 1, 1024),
-                                                    (4, 256, 8, 160, 1, 256), (4, 64, 8, 160, 1, 64),
-                                                    (4, 1024, 8, 80, 2, 512), (3, 384, 8, 40, 3, 336),
-                                                    (2, 192, 8, 40, 1, 192), (2, 80, 8, 40, 1, 80),
-                                                    # one consumer warpgroup (Nq <= 64), one step (T = 1), fewer steps than stages
-                                                    (4, 64, 8, 40, 1, 64), (2, 256, 8, 40, 2, 128), (2, 128, 4, 56, 1, 192),
-                                                    (3, 320, 8, 8, 1, 320), (2, 1024, 8, 48, 1, 1024)])
-def test_pipelined_loop_equals_serial_loop(ops, serial_loop, B, N, heads, hd, kv_div, Nk):
-    q, k, v = _inputs(B, N, heads, hd, kv_div, Nk)
+_SHAPES = [(4, 4096, 8, 40, 1, 4096), (4, 1024, 8, 80, 1, 1024), (4, 256, 8, 160, 1, 256), (4, 64, 8, 160, 1, 64),
+           (4, 1024, 8, 80, 2, 512), (3, 384, 8, 40, 3, 336), (2, 192, 8, 40, 1, 192), (2, 80, 8, 40, 1, 80),
+           # one consumer warpgroup (Nq <= 64), one step (T = 1), fewer steps than stages
+           (4, 64, 8, 40, 1, 64), (2, 256, 8, 40, 2, 128), (2, 128, 4, 56, 1, 192), (3, 320, 8, 8, 1, 320),
+           (2, 1024, 8, 48, 1, 1024)]
+
+
+# every shape on N(0, 1) data (ids without a family) and on score distributions whose exponentials underflow
+@pytest.mark.parametrize("B,N,heads,hd,kv_div,Nk,family",
+                         [pytest.param(*s, f, id="-".join(map(str, s)) + ("" if f == "flat" else "-" + f))
+                          for f in ("flat", "peaked", "rising", "tail") for s in _SHAPES])
+def test_pipelined_loop_equals_serial_loop(ops, serial_loop, B, N, heads, hd, kv_div, Nk, family):
+    q, k, v = _inputs(B, N, heads, hd, kv_div, Nk, family)
     serial_loop(True)
     ref = ops.flash_attention(q, k, v, heads, N, Nk, kv_div)
     serial_loop(False)
