@@ -20,6 +20,29 @@ def _chk_bf16(*ts):
             assert t.is_cuda and t.dtype == BF16 and t.stride(-1) == 1, (t.dtype, t.device, t.stride())
 
 
+def _chk_bias(bias, N, device, bias2=None, M=1, bias2_div=1):
+    """The epilogue reads bias[n] and bias2[(m // bias2_div) * N + n] (n < N, m < M) as float2 from raw pointers: both must
+    be fp32 on the output's device with unit column stride and 8-byte alignment, bias N entries, bias2 N columns and
+    (M - 1) // bias2_div + 1 rows, with row stride N whenever more than one row is read (a strided column slice such as
+    the per-block time embedding passes when one row serves every output row)."""
+    for name, t in (("bias", bias), ("bias2", bias2)):
+        if t is None:
+            continue
+        if t.dtype != torch.float32 or t.device != device or t.stride(-1) != 1 or t.data_ptr() % 8:
+            raise ValueError(f"{name} must be fp32 on {device} with unit column stride and 8-byte alignment, got "
+                             f"{t.dtype} on {t.device}, strides {t.stride()}")
+    if bias is not None and (bias.dim() != 1 or bias.shape[0] != N):
+        raise ValueError(f"bias must have shape ({N},), got {tuple(bias.shape)}")
+    if bias2 is not None:
+        if bias2_div < 1:
+            raise ValueError(f"bias2_div must be >= 1, got {bias2_div}")
+        rows = (M - 1) // bias2_div + 1
+        b2 = bias2 if bias2.dim() == 2 else bias2.view(1, -1) if bias2.dim() == 1 else None
+        if b2 is None or b2.shape[1] != N or b2.shape[0] < rows or (rows > 1 and b2.stride(0) != N):
+            raise ValueError(f"bias2 must be [>= {rows}, {N}] with row stride {N} when more than one row is read "
+                             f"(M = {M}, bias2_div = {bias2_div}), got shape {tuple(bias2.shape)} strides {bias2.stride()}")
+
+
 def f32_arena(vectors, device):
     """All 1-D parameters of a model (biases, norm affine) as fp32 views into ONE buffer: one concatenation and two
     casts instead of a cast kernel per parameter.  Values are rounded to the model dtype first (what ``.to(bf16)`` does
@@ -67,6 +90,7 @@ def gemm(a, w, bias=None, *, a2=None, bias2=None, bias2_div=1, scale=1.0, residu
     K2 = 0 if a2 is None else a2.shape[1]
     N = w.shape[0]
     assert w.shape[1] == K1 + K2
+    _chk_bias(bias, N, a.device, bias2, M, bias2_div)
     if geglu:
         block_n = geglu_block_n(N)
     if out is None:
@@ -110,6 +134,7 @@ def gemm_lnfold(a, wf, stats, colsum, bias, *, bias2=None, bias2_div=1, scale=1.
     M, K = a.shape
     N = wf.shape[0]
     assert wf.shape[1] == K and stats.shape == (M, 2) and colsum.shape == (N,)
+    _chk_bias(bias, N, a.device, bias2, M, bias2_div)
     if out is None:
         out = torch.empty((M, N // 2 if geglu else N), device=a.device, dtype=BF16)
     check(_ffi.lib().vx_gemm_lnfold_bf16(
@@ -133,6 +158,7 @@ def gemm_rowsums(a, w, bias=None, *, a2=None, scale=1.0, residual=None, out=None
     K2 = 0 if a2 is None else a2.shape[1]
     N = w.shape[0]
     assert w.shape[1] == K1 + K2 and N // 32 * 2 >= 2
+    _chk_bias(bias, N, a.device)
     if out is None:
         out = torch.empty((M, N), device=a.device, dtype=BF16)
     cap = rowsum_slots(N)
@@ -154,6 +180,7 @@ def gemm_lnparts(a, wf, parts, nparts, colsum, bias, eps=1e-5, *, bias2=None, bi
     M, K = a.shape
     N = wf.shape[0]
     assert wf.shape[1] == K and parts.shape[1:] == (M, 2) and 0 < nparts <= parts.shape[0] and colsum.shape == (N,)
+    _chk_bias(bias, N, a.device, bias2, M, bias2_div)
     if out is None:
         out = torch.empty((M, N // 2 if geglu else N), device=a.device, dtype=BF16)
     check(_ffi.lib().vx_gemm_lnparts_bf16(
@@ -171,6 +198,7 @@ def conv3x3(x, w, bias=None, *, bias2=None, bias2_div=1, scale=1.0, residual=Non
     NB, H, W, C = x.shape
     Cout = w.shape[0]
     assert w.shape[1] == 9 * C
+    _chk_bias(bias, Cout, x.device, bias2, NB * H * W, bias2_div)
     if out is None:
         out = torch.empty((NB * H * W, Cout), device=x.device, dtype=BF16)
     check(_ffi.lib().vx_conv3x3_bf16(
@@ -200,6 +228,7 @@ def conv3x3_s2(x, w, bias=None, *, pad_lo=1, out=None, block_n=0):
     NB, H, W, C = x.shape
     Cout = w.shape[0]
     assert w.shape[1] == 9 * C and H % 2 == 0 and W % 2 == 0
+    _chk_bias(bias, Cout, x.device)
     if out is None:
         out = torch.empty((NB * (H // 2) * (W // 2), Cout), device=x.device, dtype=BF16)
     check(_ffi.lib().vx_conv3x3s2_bf16(
@@ -237,6 +266,7 @@ def upconv3x3(x, w4, bias, out=None, block_n=0):
     NB, H, W, C = x.shape
     Cout = w4.shape[0] // 4
     assert w4.shape[1] == 4 * C
+    _chk_bias(bias, Cout, x.device)
     if out is None:
         out = torch.empty((NB * 4 * H * W, Cout), device=x.device, dtype=BF16)
     check(_ffi.lib().vx_upconv3x3_bf16(ptr(x), c_int(NB), c_int(H), c_int(W), c_int(C), ptr(w4), c_int(Cout), ptr(bias),
@@ -328,6 +358,7 @@ def gemm_ln(a, wf, colsum, bias, eps=1e-5, *, bias2=None, bias2_div=1, scale=1.0
     M, K = a.shape
     N = wf.shape[0]
     assert wf.shape[1] == K and colsum.shape == (N,) and K % 64 == 0 and K <= LN_GEMM_MAX_K
+    _chk_bias(bias, N, a.device, bias2, M, bias2_div)
     if out is None:
         out = torch.empty((M, N // 2 if geglu else N), device=a.device, dtype=BF16)
     check(_ffi.lib().vx_gemm_ln_bf16(
