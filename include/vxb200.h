@@ -169,6 +169,14 @@ int vx_skinny_linear(const float* x, int rows, int K, const void* w, const float
  * noise: ((b f),4,h,w) bf16; acc: fp32 (4, L, hw); latents: bf16 (4, L, hw) updated in place. */
 int vx_cfg_overlap_accumulate(const void* noise, int f, int hw, int L, int do_cfg, const int* win, const int* count,
                               float guidance, float* acc, void* stream);
+/* The same for n samples of one window in one launch (num_images_per_prompt): noise ((b n f),4,h,w) laid out
+ * [uncond s0..s(n-1) | cond s0..s(n-1)] (b = 2) or [s0..s(n-1)] (b = 1), f frames per block; acc fp32 (n, 4, L, hw).
+ * Per sample the rounding points and the skipped slots (win[i] = -1) are those of vx_cfg_overlap_accumulate, so sample s
+ * accumulates the bits a one-sample call on its blocks would. */
+int vx_cfg_overlap_accumulate_n(const void* noise, int n, int f, int hw, int L, int do_cfg, const int* win,
+                                const int* count, float guidance, float* acc, void* stream);
+/* vx_ddim_step is elementwise over n contiguous elements: for n samples pass latents / acc of shape (n, 4, L, hw) and
+ * n * 4 * L * hw elements; every sample gets the update a one-sample call would give it. */
 int vx_ddim_step(void* latents, const float* acc, long long n, float sqrt_a, float sqrt_1ma, float sqrt_aprev,
                  float sqrt_1maprev, void* stream);
 

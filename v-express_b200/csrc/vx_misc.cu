@@ -354,6 +354,42 @@ __global__ void cfg_overlap_kernel(const CfgArgs p) {
   }
 }
 
+// The same for n samples in one launch: noise ((b n f), 4, h, w) laid out [uncond s0..s(n-1) | cond s0..s(n-1)], each
+// block f frames; acc fp32 (n, 4, L, hw).  Every element goes through exactly the rounding points of cfg_overlap_kernel,
+// so sample s of an n-sample window accumulates the same bits as a one-sample window would.
+struct CfgNArgs {
+  const __nv_bfloat16* noise; int n, f, hw, L, do_cfg;
+  const int* win; const int* count; float g;
+  float* acc;
+};
+
+__global__ void cfg_overlap_n_kernel(const CfgNArgs p) {
+  pdl_enter();
+  const long long per = (long long)4 * p.f * p.hw;   // one sample's block of the noise
+  const long long total = per * p.n;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int px = (int)(idx % p.hw);
+    const int i = (int)((idx / p.hw) % p.f);
+    const int c = (int)((idx / ((long long)p.hw * p.f)) % 4);
+    const int s = (int)(idx / per);
+    const int fr = p.win[i];
+    if (fr < 0) continue;
+    const long long off = (long long)s * per + ((long long)i * 4 + c) * p.hw + px;
+    float v;
+    if (p.do_cfg) {
+      const float u = __bfloat162float(p.noise[off]);
+      const float cd = __bfloat162float(p.noise[(long long)p.n * per + off]);
+      v = rbf(u + rbf(p.g * rbf(cd - u)));
+    } else {
+      v = __bfloat162float(p.noise[off]);
+    }
+    v = rbf(v / (float)p.count[fr]);
+    float* a = p.acc + (((long long)s * 4 + c) * p.L + fr) * p.hw + px;
+    *a = rbf(*a + v);
+  }
+}
+
 // DDIM v-prediction step on all frames (eta = 0), bf16 rounding after every tensor op like the reference
 // (diffusers DDIMScheduler.step with fp32 scalar coefficients on model-dtype tensors, SURVEY.md B.5).
 __global__ void ddim_step_kernel(__nv_bfloat16* __restrict__ latents, const float* __restrict__ acc, long long n,
@@ -461,6 +497,18 @@ extern "C" int vx_cfg_overlap_accumulate(const void* noise, int f, int hw, int L
   CfgArgs a{(const __nv_bfloat16*)noise, f, hw, L, do_cfg, win, count, guidance, acc};
   const long long total = (long long)4 * f * hw;
   launch_k(cfg_overlap_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, a);
+  VX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vx_cfg_overlap_accumulate_n(const void* noise, int n, int f, int hw, int L, int do_cfg, const int* win,
+                                           const int* count, float guidance, float* acc, void* stream) {
+  VX_REQUIRE(n >= 1 && f >= 1 && hw >= 1 && L >= 1, "vx_cfg_overlap_accumulate_n: n=%d f=%d hw=%d L=%d", n, f, hw, L);
+  CfgNArgs a{(const __nv_bfloat16*)noise, n, f, hw, L, do_cfg, win, count, guidance, acc};
+  const long long total = (long long)n * 4 * f * hw;
+  long long blocks = (total + 255) / 256;
+  if (blocks > device_sms() * 16) blocks = device_sms() * 16;
+  launch_k(cfg_overlap_n_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, a);
   VX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

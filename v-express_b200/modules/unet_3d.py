@@ -528,14 +528,29 @@ class UNetEngine:
         return (id(self), self.bank_epoch)
 
     # ---------------------------------------------------------------- blocks
-    def _resnet(self, p, x, x2, NB, H, Wd, temb):
+    def _groupnorm(self, x, NB, HW, gamma, beta, eps, silu, x2=None, n=1):
+        """ops.groupnorm in n launches of NB // n frames, the frame count of a one-sample forward.  The GroupNorm kernels
+        pick their per-frame split (pixel chunks or cluster size, and with it the order in which partial statistics merge)
+        from the number of frames in the launch; GroupNorm is per frame, so launches of one sample's frame count keep
+        every frame's bits those of a one-sample forward."""
+        if n == 1:
+            return ops.groupnorm(x, NB, HW, gamma, beta, eps, silu, x2=x2, groups=self.groups)
+        nb = NB // n
+        out = torch.empty((NB * HW, x.shape[1] + (0 if x2 is None else x2.shape[1])), device=x.device, dtype=BF16)
+        for s in range(n):
+            r = slice(s * nb * HW, (s + 1) * nb * HW)
+            ops.groupnorm(x[r], nb, HW, gamma, beta, eps, silu, x2=None if x2 is None else x2[r], groups=self.groups,
+                          out=out[r])
+        return out
+
+    def _resnet(self, p, x, x2, NB, H, Wd, temb, n=1):
         W = self.W
         HW = H * Wd
-        h = ops.groupnorm(x, NB, HW, W[p + ".norm1.weight"], W[p + ".norm1.bias"], self.eps, True, x2=x2, groups=self.groups)
+        h = self._groupnorm(x, NB, HW, W[p + ".norm1.weight"], W[p + ".norm1.bias"], self.eps, True, x2=x2, n=n)
         off, co = self.temb_off[p + ".time_emb_proj"]
         h = ops.conv3x3(h.view(NB, H, Wd, -1), W[p + ".conv1.weight"], W[p + ".conv1.bias"],
                         bias2=temb[:, off:off + co], bias2_div=NB * HW)
-        h = ops.groupnorm(h, NB, HW, W[p + ".norm2.weight"], W[p + ".norm2.bias"], self.eps, True, groups=self.groups)
+        h = self._groupnorm(h, NB, HW, W[p + ".norm2.weight"], W[p + ".norm2.bias"], self.eps, True, n=n)
         if (p + ".conv_shortcut.weight") in W:
             sc = ops.gemm(x, W[p + ".conv_shortcut.weight"], W[p + ".conv_shortcut.bias"], a2=x2)
         else:
@@ -548,12 +563,12 @@ class UNetEngine:
         g = ops.gemm(n, W[p + ".net.0.proj.geglu_w"], W[p + ".net.0.proj.geglu_b"], geglu=True)   # GEGLU in the epilogue
         return ops.gemm(g, W[p + ".net.2.weight"], W[p + ".net.2.bias"], residual=res)
 
-    def _spatial(self, p, x, NB, HW, f, enc_flat):
+    def _spatial(self, p, x, NB, HW, f, enc_flat, n=1):
         W = self.W
         C = x.shape[1]
         heads = self.heads
         m = self.model
-        h = ops.groupnorm(x, NB, HW, W[p + ".norm.weight"], W[p + ".norm.bias"], 1e-6, False, groups=self.groups)
+        h = self._groupnorm(x, NB, HW, W[p + ".norm.weight"], W[p + ".norm.bias"], 1e-6, False, n=n)
         h, rs = self._gemm_p(h, W[p + ".proj_in.weight"], W[p + ".proj_in.bias"])
         t = p + ".transformer_blocks.0"
         block = m.get_submodule(t)
@@ -561,16 +576,18 @@ class UNetEngine:
         qkv = self._ln_gemm(h, t + ".norm1", t + ".attn1.qkv", rs=rs)
         a = ops.flash_attention(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], heads, HW, HW)
         h, rs = self._gemm_p(a, W[t + ".attn1.to_out.0.weight"], W[t + ".attn1.to_out.0.bias"], residual=h)
-        # attn1_5: reference attention, K/V from the bank (one per CFG half, shared by the f frames)
+        # attn1_5: reference attention, K/V from the bank: one K/V block per CFG half, shared by that half's n samples x f
+        # frames (the batch is [uncond s0..s(n-1) | cond s0..s(n-1)]), so the bank holds NB // (n f) blocks of Nk rows
         q = self._ln_gemm(h, t + ".norm1_5", t + ".attn1_5.to_q.weight", rs=rs)
         kv, uncond_zero = self._bank_kv(t, block)
-        Nk = kv.shape[0] // (NB // f)
-        if uncond_zero and NB == 2 * f:
+        nf = n * f
+        Nk = kv.shape[0] // (NB // nf)
+        if uncond_zero and NB == 2 * nf:
             a = torch.empty((NB * HW, C), device=self.dev, dtype=BF16)
-            a[:f * HW].zero_()
-            ops.flash_attention(q[f * HW:], kv[Nk:, :C], kv[Nk:, C:], heads, HW, Nk, kv_div=f, out=a[f * HW:])
+            a[:nf * HW].zero_()
+            ops.flash_attention(q[nf * HW:], kv[Nk:, :C], kv[Nk:, C:], heads, HW, Nk, kv_div=nf, out=a[nf * HW:])
         else:
-            a = ops.flash_attention(q, kv[:, :C], kv[:, C:], heads, HW, Nk, kv_div=f)
+            a = ops.flash_attention(q, kv[:, :C], kv[:, C:], heads, HW, Nk, kv_div=nf)
         h, rs = self._gemm_p(a, W[t + ".attn1_5.to_out.0.weight"], W[t + ".attn1_5.to_out.0.bias"],
                              scale=float(m.reference_attention_weight), residual=h)
         # attn2: audio cross-attention (5 tokens per frame)
@@ -585,11 +602,12 @@ class UNetEngine:
         h = ops.gemm(g, W[t + ".ff.net.2.weight"], W[t + ".ff.net.2.bias"], residual=h)
         return ops.gemm(h, W[p + ".proj_out.weight"], W[p + ".proj_out.bias"], residual=x)
 
-    def _motion(self, p, x, NB, HW, b, f):
+    def _motion(self, p, x, NB, HW, b, f, n=1):
+        """b: clips of f frames in the batch (all samples and CFG halves); n: samples (GroupNorm launch split)."""
         W = self.W
         p = p + ".temporal_transformer"
         C = x.shape[1]
-        h = ops.groupnorm(x, NB, HW, W[p + ".norm.weight"], W[p + ".norm.bias"], 1e-6, False, groups=self.groups)
+        h = self._groupnorm(x, NB, HW, W[p + ".norm.weight"], W[p + ".norm.bias"], 1e-6, False, n=n)
         h, rs = self._gemm_p(h, W[p + ".proj_in.weight"], W[p + ".proj_in.bias"])
         t = p + ".transformer_blocks.0"
         for i in (0, 1):
@@ -618,12 +636,16 @@ class UNetEngine:
         e = ops.skinny_linear(e, W["time_embedding.linear_2.weight"], W["time_embedding.linear_2.bias"])
         return ops.skinny_linear(e, W["temb_cat.weight"], W["temb_cat.bias"], act_in=True)
 
-    def forward_frames(self, frames, timestep, enc, kps_nhwc, kps_frame_idx, b, f, temb=None, taps=None):
-        """frames ((b f),4,h,w) bf16; enc ((b f),Lk,768); kps_nhwc [(frames) h w, C0] bf16 (rows gathered through
-        kps_frame_idx when given).  Returns ((b f),4,h,w) bf16."""
+    def forward_frames(self, frames, timestep, enc, kps_nhwc, kps_frame_idx, b, f, temb=None, taps=None, n=1):
+        """frames ((b n f),4,h,w) bf16; enc ((b n f),Lk,768); kps_nhwc [(frames) h w, C0] bf16 (rows gathered through
+        kps_frame_idx when given).  Returns ((b n f),4,h,w) bf16.
+
+        b is the CFG batch (2: uncond | cond, 1 without guidance) and n the number of samples of the same window: the batch
+        is [uncond s0..s(n-1) | cond s0..s(n-1)], f frames per block.  Every launch whose schedule depends on the batch is
+        split or shaped so that sample s comes out bit-identical to a one-sample forward of its blocks."""
         W = self.W
         NB, cin, H, Wd = frames.shape
-        assert NB == b * f
+        assert NB == b * n * f
         boc = self.boc
         if temb is None:
             temb = self.time_embedding(timestep)
@@ -640,12 +662,12 @@ class UNetEngine:
         for i in range(4):
             p = f"down_blocks.{i}"
             for j in range(2):
-                x = self._resnet(f"{p}.resnets.{j}", x, None, NB, h_, w_, temb)
+                x = self._resnet(f"{p}.resnets.{j}", x, None, NB, h_, w_, temb, n)
                 tap(f"{p}.resnets.{j}", x, h_, w_)
                 if i < 3:
-                    x = self._spatial(f"{p}.attentions.{j}", x, NB, h_ * w_, f, enc_flat)
+                    x = self._spatial(f"{p}.attentions.{j}", x, NB, h_ * w_, f, enc_flat, n)
                     tap(f"{p}.attentions.{j}", x, h_, w_)
-                x = self._motion(f"{p}.motion_modules.{j}", x, NB, h_ * w_, b, f)
+                x = self._motion(f"{p}.motion_modules.{j}", x, NB, h_ * w_, b * n, f, n)
                 tap(f"{p}.motion_modules.{j}", x, h_, w_)
                 skips.append((x, h_, w_))
             if i < 3:
@@ -653,29 +675,29 @@ class UNetEngine:
                 h_, w_ = h_ // 2, w_ // 2
                 tap(f"{p}.downsamplers.0", x, h_, w_)
                 skips.append((x, h_, w_))
-        x = self._resnet("mid_block.resnets.0", x, None, NB, h_, w_, temb)
-        x = self._spatial("mid_block.attentions.0", x, NB, h_ * w_, f, enc_flat)
-        x = self._motion("mid_block.motion_modules.0", x, NB, h_ * w_, b, f)
-        x = self._resnet("mid_block.resnets.1", x, None, NB, h_, w_, temb)
+        x = self._resnet("mid_block.resnets.0", x, None, NB, h_, w_, temb, n)
+        x = self._spatial("mid_block.attentions.0", x, NB, h_ * w_, f, enc_flat, n)
+        x = self._motion("mid_block.motion_modules.0", x, NB, h_ * w_, b * n, f, n)
+        x = self._resnet("mid_block.resnets.1", x, None, NB, h_, w_, temb, n)
         tap("mid_block", x, h_, w_)
         for i in range(4):
             p = f"up_blocks.{i}"
             for j in range(3):
                 skip, sh, sw = skips.pop()
                 assert (sh, sw) == (h_, w_)
-                x = self._resnet(f"{p}.resnets.{j}", x, skip, NB, h_, w_, temb)
+                x = self._resnet(f"{p}.resnets.{j}", x, skip, NB, h_, w_, temb, n)
                 tap(f"{p}.resnets.{j}", x, h_, w_)
                 if i > 0:
-                    x = self._spatial(f"{p}.attentions.{j}", x, NB, h_ * w_, f, enc_flat)
+                    x = self._spatial(f"{p}.attentions.{j}", x, NB, h_ * w_, f, enc_flat, n)
                     tap(f"{p}.attentions.{j}", x, h_, w_)
-                x = self._motion(f"{p}.motion_modules.{j}", x, NB, h_ * w_, b, f)
+                x = self._motion(f"{p}.motion_modules.{j}", x, NB, h_ * w_, b * n, f, n)
                 tap(f"{p}.motion_modules.{j}", x, h_, w_)
             if i < 3:
                 # Upsample3D (modules/resnet.py:53-90): nearest x2 + conv3x3, without the 4x intermediate
                 x = ops.upconv3x3(x.view(NB, h_, w_, -1), W[f"{p}.upsamplers.0.conv.weight"], W[f"{p}.upsamplers.0.conv.bias"])
                 h_, w_ = 2 * h_, 2 * w_
                 tap(f"{p}.upsamplers.0", x, h_, w_)
-        x = ops.groupnorm(x, NB, h_ * w_, W["conv_norm_out.weight"], W["conv_norm_out.bias"], self.eps, True, groups=self.groups)
+        x = self._groupnorm(x, NB, h_ * w_, W["conv_norm_out.weight"], W["conv_norm_out.bias"], self.eps, True, n=n)
         out = torch.empty((NB, self.model.config["out_channels"], H, Wd), device=self.dev, dtype=BF16)
         ops.conv_out_tc(x, NB, H, Wd, W["conv_out.packed_w"], W["conv_out.packed_b"], out)
         return out

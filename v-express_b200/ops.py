@@ -557,6 +557,16 @@ def cfg_overlap_accumulate(noise, f, hw, L, do_cfg, win, count, guidance, acc):
           "vx_cfg_overlap_accumulate")
 
 
+def cfg_overlap_accumulate_n(noise, n, f, hw, L, do_cfg, win, count, guidance, acc):
+    """cfg_overlap_accumulate for the n samples of one window: noise ((b n f),4,h,w) as [u s0..s(n-1) | c s0..s(n-1)],
+    acc fp32 (n, 4, L, hw)."""
+    assert noise.is_contiguous() and acc.is_contiguous() and acc.dtype == torch.float32
+    assert noise.numel() == (2 if do_cfg else 1) * n * f * 4 * hw and acc.numel() == n * 4 * L * hw
+    check(_ffi.lib().vx_cfg_overlap_accumulate_n(ptr(noise), c_int(n), c_int(f), c_int(hw), c_int(L), c_int(int(do_cfg)),
+                                                 ptr(win), ptr(count), c_float(guidance), ptr(acc), stream_ptr()),
+          "vx_cfg_overlap_accumulate_n")
+
+
 def ddim_step(latents, acc, sqrt_a, sqrt_1ma, sqrt_aprev, sqrt_1maprev):
     check(_ffi.lib().vx_ddim_step(ptr(latents), ptr(acc), c_ll(latents.numel()), c_float(sqrt_a), c_float(sqrt_1ma),
                                   c_float(sqrt_aprev), c_float(sqrt_1maprev), stream_ptr()), "vx_ddim_step")

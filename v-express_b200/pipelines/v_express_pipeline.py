@@ -1,6 +1,6 @@
 """H100-native ``VExpressPipeline``: drop-in for the reference's ``pipelines/v_express_pipeline.py`` denoising
 hot path (``__call__`` -> ``mean_overlap`` :409-589 and ``decode_latents`` :152-166), same call signature and
-return value ((1,3,L,H,W) fp32 on the host, values in [0,1]).
+return value ((n,3,L,H,W) fp32 on the host, values in [0,1], n = ``num_images_per_prompt``).
 
 What differs by design (SURVEY.md 0.5, 8e):
   * latents, kps features and audio tokens stay resident in HBM for the whole video (the reference shuttles every
@@ -12,7 +12,10 @@ What differs by design (SURVEY.md 0.5, 8e):
   * context windows shard over the GPUs of one box (``do_multi_devices_inference``, a dead flag in the reference):
     every rank owns a contiguous block of windows and one NCCL all-reduce per step sums the (zero-padded)
     per-frame noise-prediction buffers; the VAE decode is sharded by frame and gathered on rank 0;
-  * the VAE decodes all frames of a chunk in one batch.
+  * the VAE decodes all frames of a chunk in one batch;
+  * ``num_images_per_prompt`` = n samples of the same conditioning run through ONE UNet forward per window, batched as
+    [uncond s0..s(n-1) | cond s0..s(n-1)].  Sample i of an n-sample call is bit-identical to a one-sample call with
+    ``generator[i]`` (the reference accepts the argument but its UNet cannot run it).
 
 Out of the hot path (SURVEY.md 8f), kept as overridable hooks exactly like the reference methods:
 ``prepare_reference_latent``, ``prepare_kps_feature``, ``prepare_audio_embeddings`` and the ReferenceNet write
@@ -53,14 +56,15 @@ def partition_windows(num_windows: int, world_size: int, rank: int):
 
 
 class _GraphedUNet:
-    """One CUDA graph of ``UNetEngine.forward_frames`` per (b, f, h, w) signature with static I/O buffers."""
+    """One CUDA graph of ``UNetEngine.forward_frames`` per (b, n, f, h, w) signature with static I/O buffers of b n f
+    frames."""
 
-    def __init__(self, engine, b, f, h, w, enc_tokens, cross_dim, use_graph=True):
+    def __init__(self, engine, b, f, h, w, enc_tokens, cross_dim, use_graph=True, n=1):
         dev = engine.dev
-        self.engine, self.b, self.f = engine, b, f
-        self.frames = torch.zeros((b * f, 4, h, w), device=dev, dtype=BF16)
-        self.enc = torch.zeros((b * f, enc_tokens, cross_dim), device=dev, dtype=BF16)
-        self.kps_idx = torch.zeros((b * f,), device=dev, dtype=torch.int32)
+        self.engine, self.b, self.f, self.n = engine, b, f, n
+        self.frames = torch.zeros((b * n * f, 4, h, w), device=dev, dtype=BF16)
+        self.enc = torch.zeros((b * n * f, enc_tokens, cross_dim), device=dev, dtype=BF16)
+        self.kps_idx = torch.zeros((b * n * f,), device=dev, dtype=torch.int32)
         self.temb = None
         self.kps = None          # static copy of the channels-last kps features (address baked into the graph)
         self.graph = None
@@ -69,8 +73,9 @@ class _GraphedUNet:
         self.kps_token = None
 
     def _run(self):
+        extra = {"n": self.n} if self.n > 1 else {}          # a one-sample window is the engine's default call
         return self.engine.forward_frames(self.frames, None, self.enc, self.kps, self.kps_idx, self.b, self.f,
-                                          temb=self.temb)
+                                          temb=self.temb, **extra)
 
     def set_kps(self, kps):
         """Per video: (re)load the resident channels-last kps features; same shape keeps the captured graph."""
@@ -247,7 +252,9 @@ class VExpressPipeline:
 
     def prepare_latents(self, batch_size, num_channels_latents, width, height, video_length, dtype, device, generator,
                         latents=None):
-        """Reference :189-224: noise is drawn on the HOST in the model dtype so seeds reproduce (:514-523)."""
+        """Reference :189-224: noise is drawn on the HOST in the model dtype so seeds reproduce (:514-523).  As diffusers'
+        ``randn_tensor``: a list of generators draws sample i as its own (1, ...) tensor from ``generator[i]``, so sample i
+        of a batch equals a one-sample draw from the same generator; a single generator (or None) draws the whole batch."""
         shape = (batch_size, num_channels_latents, video_length, height // self.vae_scale_factor,
                  width // self.vae_scale_factor)
         if isinstance(generator, list) and len(generator) != batch_size:
@@ -255,7 +262,11 @@ class VExpressPipeline:
                              f"effective batch size of {batch_size}. Make sure the batch size matches the length of "
                              f"the generators.")
         if latents is None:
-            latents = torch.randn(shape, generator=generator, device="cpu", dtype=dtype)
+            if isinstance(generator, list):
+                latents = torch.cat([torch.randn((1,) + shape[1:], generator=g, device="cpu", dtype=dtype)
+                                     for g in generator])
+            else:
+                latents = torch.randn(shape, generator=generator, device="cpu", dtype=dtype)
         return latents * self.scheduler.init_noise_sigma
 
     def get_timesteps(self, num_inference_steps, strength, device):
@@ -265,16 +276,18 @@ class VExpressPipeline:
 
     # ------------------------------------------------------------------ decode
     @torch.no_grad()
-    def decode_latents(self, latents, frame_ids=None, out=None):
-        """latents (1,4,L,h,w) on the device -> frames in [0,1], fp32, ON THE DEVICE, already in the reference's output
-        layout (reference :152-166): ``out`` (3, n, H, W) (allocated when None), frame j of ``frame_ids`` (default: all)
-        written to out[:, j].  The conv_out kernel writes through the strides, so no permute pass exists."""
+    def decode_latents(self, latents, frame_ids=None, out=None, sample=0):
+        """latents (n,4,L,h,w) on the device -> frames of sample ``sample`` in [0,1], fp32, ON THE DEVICE, already in the
+        reference's output layout (reference :152-166): ``out`` (3, k, H, W) (allocated when None), frame j of
+        ``frame_ids`` (default: all) written to out[:, j].  The conv_out kernel writes through the strides, so no permute
+        pass exists.  Frames go through the VAE in chunks of ``vae_chunk`` counted from the first id, whatever the sample,
+        so every sample decodes to the bits a one-sample call gives."""
         L = latents.shape[2]
         ids = list(range(L)) if frame_ids is None else list(frame_ids)
         H, W = latents.shape[3] * self.vae_scale_factor, latents.shape[4] * self.vae_scale_factor
         if out is None:
             out = torch.empty((3, len(ids), H, W), device=latents.device, dtype=torch.float32)
-        z = latents[0].permute(1, 0, 2, 3)[ids].contiguous()                    # (n,4,h,w)
+        z = latents[sample].permute(1, 0, 2, 3)[ids].contiguous()               # (k,4,h,w)
         for i in range(0, z.shape[0], self.vae_chunk):
             n = min(self.vae_chunk, z.shape[0] - i)
             self.vae.decode_latents(z[i:i + n], out=out[:, i:i + n].permute(1, 0, 2, 3))
@@ -284,13 +297,15 @@ class VExpressPipeline:
     @torch.no_grad()
     def denoise(self, latents, kps_feature, audio_embeddings, timesteps, guidance_scale, context_frames,
                 context_overlap, context_schedule="uniform", distributed=False, callback=None, callback_steps=1):
-        """latents (1,4,L,h,w) bf16 device (updated in place and returned); kps_feature (b,C0,L,h,w) device;
+        """latents (n,4,L,h,w) bf16 device (updated in place and returned); kps_feature (b,C0,L,h,w) device;
         audio_embeddings (b,L,T,768) device.  Steps x windows with overlap averaging, CFG and DDIM
-        (reference :486-500,514-589)."""
+        (reference :486-500,514-589).  The n samples share the conditioning and step together: one UNet forward per window
+        on the batch [uncond s0..s(n-1) | cond s0..s(n-1)] whose frames all gather their kps rows from the one resident
+        copy, one CFG / overlap launch per window, one DDIM launch per step."""
         unet: UNet3DConditionModel = self.denoising_unet
         eng = unet.engine()
         dev = latents.device
-        _, _, L, h, w = latents.shape
+        n, _, L, h, w = latents.shape
         hw = h * w
         do_cfg = guidance_scale > 1.0
         b = 2 if do_cfg else 1
@@ -313,12 +328,15 @@ class VExpressPipeline:
             .permute(0, 2, 3, 4, 1).reshape(b * Lloc * hw, C0).contiguous()
         audio = audio_embeddings[:, lo:hi].to(device=dev, dtype=BF16, non_blocking=True)
         T = audio.shape[2]
-        acc = torch.zeros((4, L, hw), device=dev, dtype=torch.float32)
-        acc_x = torch.empty((4, L, hw), device=dev, dtype=BF16) if world > 1 else None
+        acc = torch.zeros((n, 4, L, hw), device=dev, dtype=torch.float32)
+        acc_x = torch.empty((n, 4, L, hw), device=dev, dtype=BF16) if world > 1 else None
         win_dev = [torch.tensor(wn, device=dev, dtype=torch.int32) for wn in windows]
         win_long = [t.long() for t in win_dev]
         plan_dev = {wi: [torch.from_numpy(r).to(dev) for r in plan[wi]] for wi in mine}
-        lat = latents[0]                                                        # (4, L, h, w) view
+        # kps row of UNet frame (bi, s, i): the CFG half's copy of window frame i, the same for every sample s
+        half_off = torch.arange(b, device=dev, dtype=torch.int32) * Lloc - lo
+        kps_idx = {wi: (win_dev[wi][None, None] + half_off[:, None, None]).expand(b, n, len(windows[wi])).reshape(-1)
+                   for wi in mine}
         # refresh the projected reference banks (outside any capture) and reuse graphs across calls while valid
         for name in eng.order:
             eng._bank_kv(name, unet.get_submodule(name))
@@ -329,25 +347,27 @@ class VExpressPipeline:
             for wi in mine:
                 window = windows[wi]
                 f = len(window)
-                key = (b, f, h, w, T, bool(self.use_cuda_graph), eng.graph_signature())
+                key = (b, n, f, h, w, T, bool(self.use_cuda_graph), eng.graph_signature())
                 g = graphs.get(key)
                 if g is None:
-                    for k_old in [k for k in graphs if k[:4] == key[:4] and k != key]:
+                    for k_old in [k for k in graphs if k[:5] == key[:5] and k != key]:
                         del graphs[k_old]                                       # stale capture of the same shape
-                    g = graphs[key] = _GraphedUNet(eng, b, f, h, w, T, audio.shape[-1], self.use_cuda_graph)
-                x = lat[:, win_long[wi]].permute(1, 0, 2, 3)                    # (f,4,h,w)
-                g.frames[:f].copy_(x)
-                if do_cfg:
-                    g.frames[f:].copy_(x)
-                g.enc.copy_(audio[:, win_long[wi] - lo].reshape(b * f, T, -1))
-                for bi in range(b):
-                    g.kps_idx[bi * f:(bi + 1) * f].copy_(win_dev[wi] + (bi * Lloc - lo))
+                    g = graphs[key] = _GraphedUNet(eng, b, f, h, w, T, audio.shape[-1], self.use_cuda_graph, n)
+                x = latents[:, :, win_long[wi]].transpose(1, 2)                 # (n,f,4,h,w)
+                g.frames.view(b, n, f, 4, h, w).copy_(x)                        # both CFG halves
+                g.enc.view(b, n, f, T, -1).copy_(audio[:, win_long[wi] - lo].unsqueeze(1))
+                g.kps_idx.copy_(kps_idx[wi])
                 if g.kps_token is not kps_nhwc:
                     g.set_kps(kps_nhwc)
                     g.kps_token = kps_nhwc
-                noise = g(temb)                                                 # ((b f),4,h,w) bf16
+                noise = g(temb)                                                 # ((b n f),4,h,w) bf16
                 for slots in plan_dev[wi]:
-                    ops.cfg_overlap_accumulate(noise, f, hw, L, do_cfg, slots, count_dev, float(guidance_scale), acc)
+                    if n == 1:
+                        ops.cfg_overlap_accumulate(noise, f, hw, L, do_cfg, slots, count_dev, float(guidance_scale),
+                                                   acc[0])
+                    else:
+                        ops.cfg_overlap_accumulate_n(noise, n, f, hw, L, do_cfg, slots, count_dev, float(guidance_scale),
+                                                     acc)
             if world > 1:
                 # every frame has at most two non-zero bf16 contributions across the ranks (its windows live on one rank
                 # or on two neighbours), so the bf16 sum is the reference's own bf16 add -- half the bytes of fp32
@@ -358,7 +378,7 @@ class VExpressPipeline:
                     torch.distributed.all_reduce(acc_x, op=torch.distributed.ReduceOp.SUM)
                     acc.copy_(acc_x)
             sa, sb, sap, sbp = ddim_coefficients(self.scheduler, int(t))
-            ops.ddim_step(lat, acc, sa, sb, sap, sbp)
+            ops.ddim_step(latents, acc, sa, sb, sap, sbp)                   # elementwise over all n samples
             if callback is not None and i % callback_steps == 0:
                 callback(i, t, latents)
         return latents
@@ -374,6 +394,8 @@ class VExpressPipeline:
                      save_gpu_memory=False, **kwargs):
         if eta != 0.0:
             raise ValueError("the DDIM hot path is deterministic (eta = 0), like the reference CLI")
+        if not isinstance(num_images_per_prompt, int) or num_images_per_prompt < 1:
+            raise ValueError(f"num_images_per_prompt must be a positive integer, got {num_images_per_prompt!r}")
         device = self.device
         do_cfg = guidance_scale > 1.0
         batch_size = 1
@@ -411,34 +433,46 @@ class VExpressPipeline:
         return self._decode_to_host(latents, distributed)
 
     def decode_to_device(self, latents, distributed):
-        """VAE decode, sharded by frame over the ranks: (3,L,H,W) fp32 on rank 0's device (None on the other ranks);
-        the shards meet over NVLink."""
-        L = latents.shape[2]
+        """VAE decode of latents (n,4,L,h,w), sharded by (sample, frame) over the ranks: (n,3,L,H,W) fp32 on rank 0's
+        device -- (3,L,H,W) when n = 1 -- and None on the other ranks; the shards meet over NVLink."""
+        n, _, L = latents.shape[:3]
         H, W = latents.shape[3] * self.vae_scale_factor, latents.shape[4] * self.vae_scale_factor
         rank, world = 0, 1
         if distributed and torch.distributed.is_available() and torch.distributed.is_initialized():
             rank, world = torch.distributed.get_rank(), torch.distributed.get_world_size()
         if world == 1:
-            return self.decode_latents(latents)
-        per = math.ceil(L / world)
-        ids = list(range(rank * per, min(L, (rank + 1) * per)))
+            if n == 1:
+                return self.decode_latents(latents)
+            out = torch.empty((n, 3, L, H, W), device=latents.device, dtype=torch.float32)
+            for s in range(n):
+                self.decode_latents(latents, out=out[s], sample=s)
+            return out
+        # rank r owns items [r per, (r + 1) per) of the sample-major (sample, frame) list: at most one run of frames per
+        # sample it touches
+        per = math.ceil(n * L / world)
+        lo, hi = rank * per, min(n * L, (rank + 1) * per)
         buf = torch.zeros((3, per, H, W), device=latents.device, dtype=torch.float32)
-        if ids:
-            self.decode_latents(latents, ids, out=buf[:, :len(ids)])
+        for s in range(n):
+            a, e = max(lo, s * L), min(hi, (s + 1) * L)
+            if a < e:
+                self.decode_latents(latents, range(a - s * L, e - s * L), out=buf[:, a - lo:e - lo], sample=s)
         gathered = [torch.empty_like(buf) for _ in range(world)] if rank == 0 else None
         torch.distributed.gather(buf, gathered, dst=0)
         if rank != 0:
             return None
-        return torch.cat(gathered, dim=1)[:, :L]
+        video = torch.cat(gathered, dim=1)[:, :n * L]
+        return video if n == 1 else video.view(3, n, L, H, W).transpose(0, 1)
 
     def _decode_to_host(self, latents, distributed):
-        """-> (1,3,L,H,W) fp32 on the host (rank 0): one device->host copy into pinned memory from torch's caching host
+        """-> (n,3,L,H,W) fp32 on the host (rank 0): one device->host copy into pinned memory from torch's caching host
         allocator (a fresh tensor per call; the block is recycled when the caller drops it)."""
         video = self.decode_to_device(latents, distributed)
         if video is None:
             return None
-        host = torch.empty((1,) + tuple(video.shape), dtype=torch.float32, pin_memory=True)
-        host[0].copy_(video, non_blocking=True)
+        if video.dim() == 4:
+            video = video.unsqueeze(0)
+        host = torch.empty(tuple(video.shape), dtype=torch.float32, pin_memory=True)
+        host.copy_(video, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         return host
 
