@@ -16,10 +16,15 @@
 //
 // One persistent CTA per SM walks output tiles (n fastest, so concurrently running CTAs share the A rows in L2).
 // Roles (384 threads = three warpgroups): warp 0 = TMA producer, warp 1 = TMA store + residual prefetch;
-// warpgroups 1 and 2 = MMA + epilogue, 64 rows of the 128-row tile each (wgmma m64nBNk16, accumulator in registers):
+// warpgroups 1 and 2 = MMA + epilogue.  Two consumer schedules:
+//   * cooperative: both warpgroups take 64 rows of every 128-row tile (wgmma m64nBNk16, BN <= 256);
+//   * ping-pong (PP, plain GEMM only, BN <= 96): warpgroup w owns the whole 128 x BN tile of every item it = w mod 2 of
+//     the CTA (two m64nBNk16 per K step).  An order barrier hands the tensor pipe over at mainloop boundaries, so one
+//     warpgroup's epilogue runs under the other's MMAs instead of stalling the pipe.
 //   wgmma -> bias/scale (+ residual read from a TMA-prefetched, 64B-swizzled smem tile) -> bf16 -> same smem
 //   tile -> TMA store (coalesced, clipped at the M/N edges by the tensor map).  While the consumers run their
-// epilogue, the producer already fills the ring with the next tile's operands.
+// epilogue, the producer already fills the ring with the next tile's operands.  Both schedules add the same products in
+// the same K order and round at the same points: their outputs are bit-identical.
 #include "vx_host.h"
 #include "vx_ptx.cuh"
 
@@ -29,6 +34,7 @@ constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 constexpr int kThreads = 384;
 constexpr int kEpiThreads = 256;
+constexpr int kPPMaxBN = 96;   // ping-pong: BN accumulators per thread; 128 spills at the 168 registers of 384 threads
 constexpr int kPanelCols = 32;                         // staging panel: 32 bf16 = 64 B rows, 64B swizzle
 constexpr int kPanelBytes = kBlockM * kPanelCols * 2;  // 8 KB
 constexpr int kSmemCap = 227 * 1024;
@@ -43,6 +49,7 @@ struct GemmArgs {
   int a_bytes;     // bytes of one A stage tile (128 rows x 128 B, or (hbox + 2) * W rows x 128 B with rr)
   int ups;         // 1: output parity classes (py, px) of conv3x3(upsample2x(x)) as four 2x2 convolutions on x (vx_upconv3x3_bf16)
   int block_n;     // wgmma N (the kernel's BN)
+  int pp;          // host only: 1 = ping-pong instantiation (pick_block_n), 0 = cooperative
   int stages;
   int nbuf;        // staging tiles (2 when shared memory allows: TMA store/residual latency fully hidden)
   int rows_valid;  // output rows covered by one tile (128 for plain; wbox*hbox*nbox for conv)
@@ -132,8 +139,9 @@ __device__ __forceinline__ uint32_t* staging_word(uint8_t* buf, int row, int col
 }
 
 // wgmma accumulator fragment of m64nBN (per thread): element 4 * g + 2 * h + e sits at row 16 * warp + lane / 4 + 8 * h,
-// column 8 * g + 2 * (lane % 4) + e of the warpgroup's 64 x BN block.
-template <int BN, bool LNF>
+// column 8 * g + 2 * (lane % 4) + e of the warpgroup's 64 x BN block.  Ping-pong: acc[mh] is the block of rows
+// [64 mh, 64 mh + 64) of the tile.
+template <int BN, bool LNF, bool PP>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapA2,
                   const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapR,
@@ -182,13 +190,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     if (p.kblocks2) tma_prefetch_desc(&mapA2);
     if (!p.out_f32) tma_prefetch_desc(&mapC);
     if (p.has_residual || p.ups) tma_prefetch_desc(&mapR);
+    // ping-pong: a stage / staging tile is consumed by one warpgroup only
+    constexpr int consumers = PP ? kEpiThreads / 2 : kEpiThreads;
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kEpiThreads / 32);   // lane 0 of every consumer warp, once its MMAs on the stage completed
+      mbar_init(&empty_bar[s], consumers / 32);   // lane 0 of every consumer warp, once its MMAs on the stage completed
     }
     for (int s = 0; s < 2; ++s) {
       mbar_init(&c_ready[s], 1);
-      mbar_init(&staged[s], kEpiThreads);
+      mbar_init(&staged[s], consumers);
     }
     for (int s = 0; s < 8; ++s) {
       mbar_init(&a_land[s], 1);
@@ -337,16 +347,28 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     }
   } else if (warp >= 4) {
     // -------------------------------------------------------------- MMA + epilogue (warpgroups 1, 2)
-    const int wg = (threadIdx.x >> 7) - 1;          // rows [64 wg, 64 wg + 64) of the tile
-    const int wrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // + 8 h: the two rows of this thread
+    static_assert(!(PP && LNF) && (!PP || BN <= kPPMaxBN), "ping-pong: plain epilogues, BN <= 96");
+    constexpr int MH = PP ? 2 : 1;                  // 64-row accumulator blocks per warpgroup
+    const int wg = (threadIdx.x >> 7) - 1;          // cooperative: rows [64 wg, 64 wg + 64) of the tile; PP: items wg mod 2
+    const int wrow = (PP ? 0 : wg * 64) + (warp & 3) * 16 + (lane >> 2);   // + 8 h (+ 64 mh): the rows of this thread
     const int cq = (lane & 3) * 2;                  // + 8 g: the column pair of this thread in column group g
-    float acc[BN / 2];
+    float acc[MH][BN / 2];
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
+    for (int mh = 0; mh < MH; ++mh)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[mh][i] = 0.f;
     float ln_mean[2] = {0.f, 0.f}, ln_rstd[2] = {1.f, 1.f};
-    for (int it = 0, t = item_at(0); t >= 0; t = item_at(++it)) {
+    // PP order barrier (named barriers 1, 2; 128 threads arrive, 128 wait): warpgroup w waits on 1 + w before the mainloop
+    // of each item but its first and, once its MMAs are issued, lets the other warpgroup go if the CTA has a next item.
+    // Every arrive is matched by exactly one wait.
+    for (int it = PP ? wg : 0, t = item_at(it); t >= 0; it += PP ? 2 : 1, t = item_at(it)) {
+      // ring position of the item's first K block: the producer fills the ring in item order, total_kb stages per item
+      const long long g0 = (long long)it * total_kb;
+      int stage = (int)(g0 % p.stages);
+      uint32_t phase = (uint32_t)((g0 / p.stages) & 1);
+      if constexpr (PP) {
+        if (it > 0) asm volatile("bar.sync %0, 256;" ::"r"(1 + wg) : "memory");
+      }
       const int tt = t % tiles_per_par;
       const int tile_n = tt % p.tiles_n, tile_m = tt / p.tiles_n;
       bool a_last = false;   // ares: last column tile of the row tile -> its MMAs release the resident K blocks
@@ -412,9 +434,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
         if constexpr (LNF) {
           if (p.ares) sa = smem_u32(smem + kb * (kBlockM * kBlockK * 2));
         }
-        sa += (uint32_t)(wg * 64 * 128);
+        if constexpr (!PP) sa += (uint32_t)(wg * 64 * 128);
         wgmma_fence();
-        if (p.rr) {
+        if (!PP && p.rr) {
           // tap dy reads the 128 tile rows that start dy image rows (W x 128 B, a multiple of the 1024-B swizzle atom)
           // into the A box, against its own W tile
 #pragma unroll
@@ -423,14 +445,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
             const uint64_t db = make_smem_desc(sb + (uint32_t)(dyi * b_bytes), 16, 1024, SWZ_128B);
 #pragma unroll
             for (int k = 0; k < kBlockK / 16; ++k)   // +32 bytes per K step = +2 in the (addr >> 4) field
-              Wgmma<BN>::template ss<0, 0>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | dyi | k) != 0);
+              Wgmma<BN>::template ss<0, 0>(acc[0], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | dyi | k) != 0);
           }
         } else {
-          const uint64_t da = make_smem_desc(sa, 16, 1024, SWZ_128B);
           const uint64_t db = make_smem_desc(sb, 16, 1024, SWZ_128B);
 #pragma unroll
           for (int k = 0; k < kBlockK / 16; ++k)
-            Wgmma<BN>::template ss<0, 0>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) != 0);
+#pragma unroll
+            for (int mh = 0; mh < MH; ++mh) {   // PP: rows 64 mh.. of the A tile, 64 x 128 B further on
+              const uint64_t da = make_smem_desc(sa + (uint32_t)(mh * 64 * 128), 16, 1024, SWZ_128B);
+              Wgmma<BN>::template ss<0, 0>(acc[mh], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) != 0);
+            }
         }
         wgmma_commit();
         wgmma_wait<1>();                              // the MMAs of the previous stage have completed: release it
@@ -441,8 +466,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
           phase ^= 1;
         }
       }
+      if constexpr (PP) {   // MMAs issued: the other warpgroup's mainloop queues behind them while this one finishes
+        if (item_at(it + 1) >= 0) asm volatile("bar.arrive %0, 256;" ::"r"(1 + (wg ^ 1)) : "memory");
+      }
       wgmma_wait<0>();
-      wgmma_fence_regs(acc);
+#pragma unroll
+      for (int mh = 0; mh < MH; ++mh) wgmma_fence_regs(acc[mh]);
       if (lane == 0) {
         mbar_arrive(&empty_bar[prev]);
         if constexpr (LNF) {
@@ -456,115 +485,120 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
       if (!p.out_f32) mbar_wait(&c_ready[sb], (uint32_t)((it / p.nbuf) & 1));
       uint8_t* buf = sC + sb * buf_bytes;
       const int nbase = tile_n * BN;  // accumulator column base (bias index)
-      long long m[2];
-      bool row_ok[2];
-      const float* b2[2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = wrow + 8 * h;
-        m[h] = (long long)tile_m * p.rows_valid + r;
-        row_ok[h] = r < p.rows_valid && m[h] < p.M;
-        b2[h] = p.bias2 ? p.bias2 + (row_ok[h] ? (m[h] / p.bias2_div) : 0) * (long long)p.N : nullptr;
-        if constexpr (LNF) {
-          if (p.ares) {
-          } else if (p.ln_parts) {
-            if (row_ok[h]) {
-              float s1 = 0.f, s2 = 0.f;
-              for (int j = 0; j < p.ln_nparts; ++j) {
-                const float2 v = __ldg(p.ln_parts + (long long)j * p.ln_pstride + m[h]);
-                s1 += v.x;
-                s2 += v.y;
-              }
-              ln_mean[h] = s1 * p.ln_invK;
-              ln_rstd[h] = rsqrtf(fmaxf(fmaf(-ln_mean[h], ln_mean[h], s2 * p.ln_invK), 0.f) + p.ln_eps);
-            }
-          } else if (row_ok[h]) {
-            const float2 st = *reinterpret_cast<const float2*>(p.ln_stats + 2 * m[h]);
-            ln_mean[h] = st.x;
-            ln_rstd[h] = st.y;
-          }
-        }
-      }
-      if (p.geglu) {
-        constexpr int G2 = BN / 16;   // value column groups; the gate of group g is group g + G2
+      for (int mh = 0; mh < MH; ++mh) {   // PP: the two 64-row blocks one after the other (fewer live registers)
+        const int rbase = wrow + 64 * mh;
+        float (&ac)[BN / 2] = acc[mh];
+        long long m[2];
+        bool row_ok[2];
+        const float* b2[2];
 #pragma unroll
-        for (int g = 0; g < G2; ++g) {
-          const int nl = g * 8 + cq;
-          const int nv = nbase + nl, ng = nbase + BN / 2 + nl;
-          const float2 bv = p.bias ? *reinterpret_cast<const float2*>(p.bias + nv) : make_float2(0.f, 0.f);
-          const float2 bg = p.bias ? *reinterpret_cast<const float2*>(p.bias + ng) : make_float2(0.f, 0.f);
-          float2 sv = make_float2(0.f, 0.f), sg = make_float2(0.f, 0.f);
+        for (int h = 0; h < 2; ++h) {
+          const int r = rbase + 8 * h;
+          m[h] = (long long)tile_m * p.rows_valid + r;
+          row_ok[h] = r < p.rows_valid && m[h] < p.M;
+          b2[h] = p.bias2 ? p.bias2 + (row_ok[h] ? (m[h] / p.bias2_div) : 0) * (long long)p.N : nullptr;
           if constexpr (LNF) {
-            sv = *reinterpret_cast<const float2*>(p.ln_colsum + nv);
-            sg = *reinterpret_cast<const float2*>(p.ln_colsum + ng);
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float v0 = acc[4 * g + 2 * h], v1 = acc[4 * g + 2 * h + 1];
-            float g0 = acc[4 * (g + G2) + 2 * h], g1 = acc[4 * (g + G2) + 2 * h + 1];
-            if constexpr (LNF) {
-              v0 = ln_rstd[h] * (v0 - ln_mean[h] * sv.x);
-              v1 = ln_rstd[h] * (v1 - ln_mean[h] * sv.y);
-              g0 = ln_rstd[h] * (g0 - ln_mean[h] * sg.x);
-              g1 = ln_rstd[h] * (g1 - ln_mean[h] * sg.y);
-            }
-            const float f0 = (v0 + bv.x) * gelu_erf(g0 + bg.x), f1 = (v1 + bv.y) * gelu_erf(g1 + bg.y);
-            *staging_word(buf, wrow + 8 * h, nl) = pack_bf16(f0, f1);
-          }
-        }
-      } else {
-        float rs_sum[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, rs_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][column half]
-#pragma unroll
-        for (int g = 0; g < BN / 8; ++g) {
-          const int nl = g * 8 + cq;
-          const int n = nbase + nl;
-          const float2 bv = p.bias ? *reinterpret_cast<const float2*>(p.bias + n) : make_float2(0.f, 0.f);
-          float2 cs = make_float2(0.f, 0.f);
-          if constexpr (LNF) cs = *reinterpret_cast<const float2*>(p.ln_colsum + n);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float f0 = acc[4 * g + 2 * h], f1 = acc[4 * g + 2 * h + 1];
-            if constexpr (LNF) {
-              f0 = ln_rstd[h] * (f0 - ln_mean[h] * cs.x);
-              f1 = ln_rstd[h] * (f1 - ln_mean[h] * cs.y);
-            }
-            f0 += bv.x;
-            f1 += bv.y;
-            if (b2[h]) {
-              const float2 t2 = *reinterpret_cast<const float2*>(b2[h] + n);
-              f0 += t2.x;
-              f1 += t2.y;
-            }
-            f0 *= p.scale;
-            f1 *= p.scale;
-            if (p.out_f32) {
-              if (row_ok[h]) *reinterpret_cast<float2*>(p.out32 + m[h] * p.ldc + n) = make_float2(f0, f1);
-              continue;
-            }
-            uint32_t* sp = staging_word(buf, wrow + 8 * h, nl);
-            if (p.has_residual) {
-              const float2 r2 = unpack_bf16(*sp);
-              f0 += r2.x;
-              f1 += r2.y;
-            }
-            const uint32_t pk = pack_bf16(f0, f1);
-            *sp = pk;
-            if (p.rs_out) {
-              const float2 t2 = unpack_bf16(pk);
-              const int half = nl >= BN / 2;
-              rs_sum[h][half] += t2.x + t2.y;
-              rs_sq[h][half] = fmaf(t2.x, t2.x, fmaf(t2.y, t2.y, rs_sq[h][half]));
+            if (p.ares) {
+            } else if (p.ln_parts) {
+              if (row_ok[h]) {
+                float s1 = 0.f, s2 = 0.f;
+                for (int j = 0; j < p.ln_nparts; ++j) {
+                  const float2 v = __ldg(p.ln_parts + (long long)j * p.ln_pstride + m[h]);
+                  s1 += v.x;
+                  s2 += v.y;
+                }
+                ln_mean[h] = s1 * p.ln_invK;
+                ln_rstd[h] = rsqrtf(fmaxf(fmaf(-ln_mean[h], ln_mean[h], s2 * p.ln_invK), 0.f) + p.ln_eps);
+              }
+            } else if (row_ok[h]) {
+              const float2 st = *reinterpret_cast<const float2*>(p.ln_stats + 2 * m[h]);
+              ln_mean[h] = st.x;
+              ln_rstd[h] = st.y;
             }
           }
         }
-        if (p.rs_out) {
+        if (p.geglu) {
+          constexpr int G2 = BN / 16;   // value column groups; the gate of group g is group g + G2
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-              const float s1 = quad_sum(rs_sum[h][half]), s2 = quad_sum(rs_sq[h][half]);
-              if ((lane & 3) == 0 && row_ok[h]) p.rs_out[(long long)(tile_n * 2 + half) * p.rs_stride + m[h]] = make_float2(s1, s2);
+          for (int g = 0; g < G2; ++g) {
+            const int nl = g * 8 + cq;
+            const int nv = nbase + nl, ng = nbase + BN / 2 + nl;
+            const float2 bv = p.bias ? *reinterpret_cast<const float2*>(p.bias + nv) : make_float2(0.f, 0.f);
+            const float2 bg = p.bias ? *reinterpret_cast<const float2*>(p.bias + ng) : make_float2(0.f, 0.f);
+            float2 sv = make_float2(0.f, 0.f), sg = make_float2(0.f, 0.f);
+            if constexpr (LNF) {
+              sv = *reinterpret_cast<const float2*>(p.ln_colsum + nv);
+              sg = *reinterpret_cast<const float2*>(p.ln_colsum + ng);
             }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float v0 = ac[4 * g + 2 * h], v1 = ac[4 * g + 2 * h + 1];
+              float g0 = ac[4 * (g + G2) + 2 * h], g1 = ac[4 * (g + G2) + 2 * h + 1];
+              if constexpr (LNF) {
+                v0 = ln_rstd[h] * (v0 - ln_mean[h] * sv.x);
+                v1 = ln_rstd[h] * (v1 - ln_mean[h] * sv.y);
+                g0 = ln_rstd[h] * (g0 - ln_mean[h] * sg.x);
+                g1 = ln_rstd[h] * (g1 - ln_mean[h] * sg.y);
+              }
+              const float f0 = (v0 + bv.x) * gelu_erf(g0 + bg.x), f1 = (v1 + bv.y) * gelu_erf(g1 + bg.y);
+              *staging_word(buf, rbase + 8 * h, nl) = pack_bf16(f0, f1);
+            }
+          }
+        } else {
+          float rs_sum[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, rs_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][column half]
+#pragma unroll
+          for (int g = 0; g < BN / 8; ++g) {
+            const int nl = g * 8 + cq;
+            const int n = nbase + nl;
+            const float2 bv = p.bias ? *reinterpret_cast<const float2*>(p.bias + n) : make_float2(0.f, 0.f);
+            float2 cs = make_float2(0.f, 0.f);
+            if constexpr (LNF) cs = *reinterpret_cast<const float2*>(p.ln_colsum + n);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float f0 = ac[4 * g + 2 * h], f1 = ac[4 * g + 2 * h + 1];
+              if constexpr (LNF) {
+                f0 = ln_rstd[h] * (f0 - ln_mean[h] * cs.x);
+                f1 = ln_rstd[h] * (f1 - ln_mean[h] * cs.y);
+              }
+              f0 += bv.x;
+              f1 += bv.y;
+              if (b2[h]) {
+                const float2 t2 = *reinterpret_cast<const float2*>(b2[h] + n);
+                f0 += t2.x;
+                f1 += t2.y;
+              }
+              f0 *= p.scale;
+              f1 *= p.scale;
+              if (p.out_f32) {
+                if (row_ok[h]) *reinterpret_cast<float2*>(p.out32 + m[h] * p.ldc + n) = make_float2(f0, f1);
+                continue;
+              }
+              uint32_t* sp = staging_word(buf, rbase + 8 * h, nl);
+              if (p.has_residual) {
+                const float2 r2 = unpack_bf16(*sp);
+                f0 += r2.x;
+                f1 += r2.y;
+              }
+              const uint32_t pk = pack_bf16(f0, f1);
+              *sp = pk;
+              if (!PP && p.rs_out) {
+                const float2 t2 = unpack_bf16(pk);
+                const int half = nl >= BN / 2;
+                rs_sum[h][half] += t2.x + t2.y;
+                rs_sq[h][half] = fmaf(t2.x, t2.x, fmaf(t2.y, t2.y, rs_sq[h][half]));
+              }
+            }
+          }
+          if (!PP && p.rs_out) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int half = 0; half < 2; ++half) {
+                const float s1 = quad_sum(rs_sum[h][half]), s2 = quad_sum(rs_sq[h][half]);
+                if ((lane & 3) == 0 && row_ok[h]) p.rs_out[(long long)(tile_n * 2 + half) * p.rs_stride + m[h]] = make_float2(s1, s2);
+              }
+          }
         }
       }
       if (!p.out_f32) {
@@ -578,7 +612,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
 // A/B switches (bring-up only) are read ONCE per process: the launch path never touches the environment
 // (the sweep tools re-read them through vx_gemm_reload_env).
 struct GemmEnv {
-  int stages, nbuf, bn, verbose, conv_rr;
+  int stages, nbuf, bn, verbose, conv_rr, pp;
   static int geti(const char* name, int dflt) {
     const char* s = getenv(name);
     return s ? atoi(s) : dflt;
@@ -589,6 +623,7 @@ struct GemmEnv {
     bn = geti("VX_GEMM_BN", 0);
     verbose = geti("VX_GEMM_VERBOSE", 0);
     conv_rr = geti("VX_CONV_RR", 1);
+    pp = geti("VX_GEMM_PP", -1);   // -1: schedule from the shape; 0: cooperative; 1: ping-pong wherever the kernel has it
   }
 };
 static GemmEnv& gemm_env() {
@@ -604,15 +639,37 @@ static bool bn_supported(int bn) {
   }
 }
 
-// Pick the wgmma N: among the supported widths (multiples of `gran` that divide N), minimise
-//   waves(tiles) x (cycles per K block x K blocks + epilogue), with cycles per 128 x bn x 64 block = max(MMA 4 bn,
-//   shared-memory operand feed 128 + 2 bn at 128 B/clk: A once, W once per consumer warpgroup) + issue overhead.
-static int pick_block_n(long long tiles_m, int N, int gran, int total_kb) {
+// column-tile widths the ping-pong schedule is instantiated for
+static bool pp_bn_supported(int bn) { return bn == 32 || bn == 64 || bn == 96; }
+
+// Pick the schedule and the wgmma N (only `fixed_bn` if it is set).
+// Ping-pong (where `pp_ok`): the widest ping-pong width that divides N and is a multiple of `gran`.  By default only bn 96.
+//   Measured with tools/gemm_ab.py (H100 SXM, DESIGN section 9): at the same 128 x bn tile, ping-pong is x1.05 to x1.23 faster
+//   than cooperative on every plain-GEMM shape of the benchmark forward, so the schedule pays wherever it runs.  Against the
+//   wider cooperative tile the cost model below picks, only bn 96 wins (the qkv projections, N = 3 C: x1.03 to x1.19).  Bn 64
+//   moves more operand bytes per FLOP from L2 and loses to the cooperative bn 160 / 256 tile on every shape with M >= 8192
+//   (x0.79 to x0.99).  VX_GEMM_PP=1 allows bn 64 / 32 too.
+// Cooperative: among the supported widths (multiples of `gran` that divide N), minimise waves(tiles) x (cycles per K
+//   block x K blocks + epilogue).  Cycles per 128 x bn x 64 block = max(MMA 4 bn, shared-memory operand feed 128 + 2 bn at
+//   128 B/clk: A once, W once per consumer warpgroup) + issue overhead.
+// VX_GEMM_PP=0 never picks ping-pong.
+static int pick_block_n(long long tiles_m, int N, int gran, int total_kb, int fixed_bn = 0, bool pp_ok = false,
+                        int* pp = nullptr) {
+  const int mode = gemm_env().pp;
+  if (pp) *pp = 0;
+  if (pp_ok && mode != 0) {
+    for (int bn = kPPMaxBN; bn >= 32; bn -= 32) {
+      if (mode == -1 && bn != kPPMaxBN) break;
+      if (N % bn || bn % gran || (fixed_bn > 0 && bn != fixed_bn)) continue;
+      if (pp) *pp = 1;
+      return bn;
+    }
+  }
   const int sms = device_sms();
   int best = 0;
   double best_cost = 1e30;
   for (int bn = 256; bn >= gran; bn -= gran) {
-    if (N % bn || !bn_supported(bn)) continue;
+    if (N % bn || !bn_supported(bn) || (fixed_bn > 0 && bn != fixed_bn)) continue;
     const long long items = tiles_m * (N / bn);
     const double waves = (double)((items + sms - 1) / sms);
     const double cyc = (4.0 * bn > 128.0 + 2.0 * bn) ? 4.0 * bn : 128.0 + 2.0 * bn;
@@ -625,30 +682,40 @@ static int pick_block_n(long long tiles_m, int N, int gran, int total_kb) {
   return best;
 }
 
-template <int BN, bool LNF>
+template <int BN, bool LNF, bool PP>
 static cudaError_t launch_bn(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mB, const CUtensorMap& mR,
                              const CUtensorMap& mC, const GemmArgs& a, int grid, size_t smem, cudaStream_t st) {
   static bool configured = false;
   if (!configured) {
-    const cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, LNF>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap);
+    const cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, LNF, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap);
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  return launch_k((gemm_wgmma_kernel<BN, LNF>), dim3(grid), dim3(kThreads), smem, st, mA, mA2, mB, mR, mC, a);
+  return launch_k((gemm_wgmma_kernel<BN, LNF, PP>), dim3(grid), dim3(kThreads), smem, st, mA, mA2, mB, mR, mC, a);
 }
 
 template <bool LNF>
 static cudaError_t launch_lnf(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mB, const CUtensorMap& mR,
                               const CUtensorMap& mC, const GemmArgs& a, int grid, size_t smem, cudaStream_t st) {
+  if constexpr (!LNF) {
+    if (a.pp) {
+      switch (a.block_n) {
+        case 32: return launch_bn<32, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        case 64: return launch_bn<64, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        case 96: return launch_bn<96, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        default: return cudaErrorInvalidValue;
+      }
+    }
+  }
   switch (a.block_n) {
-    case 16: return launch_bn<16, LNF>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 32: return launch_bn<32, LNF>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 64: return launch_bn<64, LNF>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 96: return launch_bn<96, LNF>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 128: return launch_bn<128, LNF>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 160: return launch_bn<160, LNF>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 192: return launch_bn<192, LNF>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 256: return launch_bn<256, LNF>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 16: return launch_bn<16, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 32: return launch_bn<32, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 64: return launch_bn<64, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 96: return launch_bn<96, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 128: return launch_bn<128, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 160: return launch_bn<160, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 192: return launch_bn<192, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 256: return launch_bn<256, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
     default: return cudaErrorInvalidValue;
   }
 }
@@ -684,14 +751,18 @@ static int launch(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorM
   while (stages > 2 && (size_t)stages * stage_bytes + (size_t)nbuf * buf_bytes > cap) --stages;
   a.stages = stages;
   a.nbuf = nbuf;
+  // ping-pong: warpgroup b owns staging tile b (a shared tile would let one warpgroup run a phase ahead of the other)
+  if (a.pp && !a.out_f32 && nbuf != 2) a.pp = 0;
   const size_t smem = (size_t)stages * stage_bytes + (size_t)nbuf * buf_bytes + kSmemReserve + (a.ares ? (size_t)a.ares_bytes : 0);
   VX_REQUIRE(smem <= (size_t)kSmemCap, "vx_gemm: %zu bytes of shared memory needed (bn=%d, K blocks=%d)", smem, a.block_n,
              a.kblocks1);
   if (gemm_env().verbose)
-    fprintf(stderr, "[vx_gemm] M=%d N=%d kb=%d taps=%d bn=%d stages=%d nbuf=%d tiles=%dx%d\n", a.M, a.N, total_kb, a.taps,
-            a.block_n, stages, nbuf, a.tiles_m, a.tiles_n);
+    fprintf(stderr, "[vx_gemm] M=%d N=%d kb=%d taps=%d bn=%d pp=%d stages=%d nbuf=%d tiles=%dx%d\n", a.M, a.N, total_kb,
+            a.taps, a.block_n, a.pp, stages, nbuf, a.tiles_m, a.tiles_n);
   const int npar = a.ups ? 4 : 1;
   const bool lnf = a.ln_stats != nullptr || a.ln_parts != nullptr || a.ares;
+  VX_REQUIRE(!a.pp || (a.taps == 1 && !lnf && !a.rs_out && pp_bn_supported(a.block_n)), "vx_gemm: no ping-pong kernel for bn=%d",
+             a.block_n);
   const long long tiles = a.ares ? a.tiles_m : (long long)a.tiles_m * a.tiles_n * npar;
   const int grid = tiles < device_sms() ? (int)tiles : device_sms();
   if (lnf) VX_CHECK_CUDA((launch_lnf<true>(mA, mA2, mB, mR, mC, a, grid, smem, st)));
@@ -777,8 +848,14 @@ static int gemm_entry(const void* A, long long lda, int K1, const void* A2, long
           }
     }
     VX_REQUIRE(block_n > 0, "vx_gemm_ln_bf16: no column tile of N=%d fits beside the resident K=%d tile", N, K1);
-  } else if (block_n <= 0) {
-    block_n = pick_block_n(tiles_m, N, gran, total_kb);
+  }
+  // ping-pong covers the plain producer with the linear / GEGLU / fp32 epilogues (not the LayerNorm or row-sum variants)
+  const bool pp_ok = !ln_colsum && !(rs && rs->out);
+  int pp = 0;
+  if (!ares) {
+    const int fixed = block_n;
+    block_n = pick_block_n(tiles_m, N, gran, total_kb, fixed, pp_ok, &pp);
+    if (!block_n) block_n = fixed;   // not a width the picker knows: rejected below
   }
   VX_REQUIRE(block_n >= gran && block_n % gran == 0 && block_n <= 256 && N % block_n == 0,
              "vx_gemm_bf16: block_n=%d invalid for N=%d", block_n, N);
@@ -815,6 +892,7 @@ static int gemm_entry(const void* A, long long lda, int K1, const void* A2, long
   a.kblocks2 = (K2 + kBlockK - 1) / kBlockK;
   a.taps = 1;
   a.block_n = block_n;
+  a.pp = pp;
   a.rows_valid = kBlockM;
   a.W = a.H = 1;
   a.tiles_m = tiles_m;

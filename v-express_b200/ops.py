@@ -68,11 +68,12 @@ def geglu_block_n(N):
     raise ValueError(f"GEGLU GEMM needs N % 64 == 0, got {N}")
 
 
-def pack_geglu(w, bias):
+def pack_geglu(w, bias, bn=None):
     """Reorder the rows of FeedForward.net.0.proj ([2*inner, K]: value rows then gate rows) so that every
-    block_n-wide output tile holds block_n/2 value columns followed by the matching block_n/2 gate columns."""
+    block_n-wide output tile holds block_n/2 value columns followed by the matching block_n/2 gate columns
+    (block_n = bn, default geglu_block_n(N); gemm(geglu=True) needs the same block_n)."""
     N = w.shape[0]
-    bn = geglu_block_n(N)
+    bn = bn or geglu_block_n(N)
     inner, hb = N // 2, bn // 2
     idx = torch.arange(N, device=w.device).view(N // bn, 2, hb)
     t = torch.arange(N // bn, device=w.device).view(-1, 1)
@@ -84,14 +85,15 @@ def pack_geglu(w, bias):
 def gemm(a, w, bias=None, *, a2=None, bias2=None, bias2_div=1, scale=1.0, residual=None, out=None, block_n=0,
          out_f32=False, geglu=False):
     """out = (concat(a, a2) @ w.T + bias + bias2[row // bias2_div]) * scale + residual  (bf16, or fp32 if out_f32).
-    geglu=True: w/bias packed by pack_geglu; out[:, j] = (v_j + b) * gelu(g_j + b) with N/2 columns."""
+    geglu=True: w/bias packed by pack_geglu (at block_n, default geglu_block_n(N)); out[:, j] = (v_j + b) * gelu(g_j + b)
+    with N/2 columns."""
     _chk_bf16(a, w, a2, residual, None if out_f32 else out)
     M, K1 = a.shape
     K2 = 0 if a2 is None else a2.shape[1]
     N = w.shape[0]
     assert w.shape[1] == K1 + K2
     _chk_bias(bias, N, a.device, bias2, M, bias2_div)
-    if geglu:
+    if geglu and not block_n:
         block_n = geglu_block_n(N)
     if out is None:
         out = torch.empty((M, N // 2 if geglu else N), device=a.device, dtype=torch.float32 if out_f32 else BF16)
