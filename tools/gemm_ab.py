@@ -1,21 +1,23 @@
-"""A/B timing of the two GEMM consumer schedules (cooperative vs ping-pong) on the GEMM / convolution shapes of one UNet
-forward of the benchmark workload (b = 2 CFG halves x f = 16 frames, 64x64 latents: 32 frames per launch).
+"""A/B timing of the GEMM consumer schedules (cooperative, ping-pong at each width) on the GEMM / convolution shapes of
+one UNet forward of the benchmark workload (b = 2 CFG halves x f = 16 frames, 64x64 latents: 32 frames per launch).
 
-    python tools/gemm_ab.py [--min-ms 300] [--rounds 3] [--plan] [--json FILE]
+    python tools/gemm_ab.py [--min-ms 300] [--rounds 3] [--widths 64,96,128,160] [--baseline-lib LIB] [--plan] [--json FILE]
 
 The shape list restates the launches `UNetEngine.forward_frames` issues (4 down levels of 320 / 640 / 1280 / 1280 channels,
 the mid block, 4 up levels with 3 resnets each; spatial transformers at the 64 / 32 / 16 levels, motion modules
-everywhere).  Per plain-GEMM shape three arms alternate, A B C A B C, `--rounds` times each:
-  old   cooperative schedule (VX_GEMM_PP=0) at the column tile the library picks for it;
-  new   ping-pong schedule (VX_GEMM_PP=1) at the column tile the library picks for it (<= 96);
-  same  cooperative schedule at the ping-pong arm's column tile: the same 128 x bn tile, operand traffic and accumulators
-        per thread as `new`, so new against same isolates the schedule, old against same the tile width.
+everywhere).  Per shape these arms alternate, arm by arm, `--rounds` times:
+  parent  (with --baseline-lib: a libvxb200.so built from an earlier commit) that library's default choice;
+  coop    cooperative schedule (VX_GEMM_PP=0) at the column tile the cost model picks for it;
+  pp<bn>  ping-pong schedule (VX_GEMM_PP=1) at column tile bn, for every width in --widths that divides N (GEGLU: and is a
+          multiple of 64); a stride-1 convolution uses row reuse where two ring stages fit beside two staging tiles;
+  default the library's default rule (timed only when it differs from every arm above).
+GEGLU weights are packed for each arm's tile; the parent, coop and default arms use the 256-column packing.
 One sample is as many back-to-back launches as fill at least `--min-ms` between two CUDA events; the SM clock is read by a
-thread while that window runs.  GEGLU weights are packed for each arm's tile.  Prints ms per launch (median over rounds,
-with the spread), TFLOP/s (2 M N K), the L2 -> shared-memory operand bytes per FLOP of the tile ((128 + bn) / (128 bn):
-every K block moves a 128-row A box and a bn-row W box), the ratios, which schedule the default rule picks, and whether
-the outputs are bit-identical.  The convolutions have one schedule (cooperative) and are timed once per round.  The card
-name, power limit and the median sampled SM clock are printed with the table.  Inputs come from a seed.
+thread while that window runs.  Prints ms per launch (median over rounds, with the spread), TFLOP/s (2 M N K), the
+L2 -> shared-memory operand bytes per FLOP of the tile ((128 + bn) / (128 bn): every K block moves a 128-row A box and a
+bn-row W box), whether every arm's output is bit-identical to coop's, and per forward the sum over launches for the
+parent, coop, the default rule and the fastest arm of every shape.  The card name, power limit and the median sampled SM
+clock are printed with the table.  Inputs come from a seed.
 `--plan` prints the shape / FLOP table and stops; timing without a CUDA device is an error."""
 import argparse
 import json
@@ -101,6 +103,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--plan", action="store_true")
     ap.add_argument("--json", default=None, help="also write the table to this file")
+    ap.add_argument("--widths", default="64,96,128,160", help="ping-pong column tiles to time")
+    ap.add_argument("--baseline-lib", default=None, help="libvxb200.so of an earlier build, timed as the parent arm")
     args = ap.parse_args()
 
     shapes = unique_shapes()
@@ -127,10 +131,10 @@ def main():
                 os.environ.pop(k, None)
             else:
                 os.environ[k] = str(v)
-        lib.vx_gemm_reload_env()
+        _ffi.lib().vx_gemm_reload_env()   # the library the next arm runs on
 
     def launch_info(run):
-        """(bn, pp) of one launch, from the VX_GEMM_VERBOSE log on fd 2"""
+        """(bn, pp, rr) of one launch, from the VX_GEMM_VERBOSE log on fd 2 (rr: None where the log does not say)"""
         set_env(VX_GEMM_VERBOSE=1)
         sys.stderr.flush()
         saved = os.dup(2)
@@ -145,8 +149,8 @@ def main():
             f.seek(0)
             log = f.read().decode()
         set_env(VX_GEMM_VERBOSE=None)
-        m = re.findall(r"bn=(\d+) pp=(\d+)", log)
-        return (int(m[-1][0]), int(m[-1][1])) if m else (0, 0)
+        m = re.findall(r"bn=(\d+) pp=(\d+)(?: rr=(\d+))?", log)
+        return (int(m[-1][0]), int(m[-1][1]), int(m[-1][2]) if m[-1][2] else None) if m else (0, 0, None)
 
     def window(run, n, sample):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -170,108 +174,105 @@ def main():
         n = max(3, int(args.min_ms / max(one, 1e-3)) + 1)
         return window(run, n, True)
 
+    baseline = None
+    if args.baseline_lib:
+        import ctypes
+        baseline = ctypes.CDLL(os.path.abspath(args.baseline_lib))
+        baseline.vx_last_error.restype = ctypes.c_char_p
+    widths = [int(w) for w in args.widths.split(",")]
     bpf = lambda bn: (128.0 + bn) / (128.0 * bn)
     rows, clocks = [], []
-    tot = {"old": 0.0, "new": 0.0, "default": 0.0}
+    tot = {"parent": 0.0, "coop": 0.0, "default": 0.0, "best": 0.0}
     for (kind, M, N, K), cnt in shapes:
         gen = torch.Generator(device="cuda").manual_seed(M + 7 * N + 13 * K)
         fl = 2.0 * M * N * K
-        conv = kind.startswith("conv") or kind.startswith("upconv")
-        if conv:
+        geglu = "geglu" in kind
+        if kind.startswith(("conv", "upconv")):
             side = int(round((M / FRAMES) ** 0.5))
             if kind == "upconv3x3":
                 C = K // 4
                 x = torch.randn(FRAMES, side // 2, side // 2, C, device="cuda", generator=gen).bfloat16()
                 w = (torch.randn(4 * N, K, device="cuda", generator=gen) / K ** 0.5).bfloat16()
                 bias = torch.randn(N, device="cuda", generator=gen)
-                run = lambda: ops.upconv3x3(x, w, bias)
+                make = lambda bn: (lambda: ops.upconv3x3(x, w, bias, block_n=bn))
             elif kind == "conv3x3 s2":
                 C = K // 9
                 x = torch.randn(FRAMES, 2 * side, 2 * side, C, device="cuda", generator=gen).bfloat16()
                 w = (torch.randn(N, K, device="cuda", generator=gen) / K ** 0.5).bfloat16()
                 bias = torch.randn(N, device="cuda", generator=gen)
-                run = lambda: ops.conv3x3_s2(x, w, bias)
+                make = lambda bn: (lambda: ops.conv3x3_s2(x, w, bias, block_n=bn))
             else:
                 C = K // 9
                 x = torch.randn(FRAMES, side, side, C, device="cuda", generator=gen).bfloat16()
                 w = (torch.randn(N, K, device="cuda", generator=gen) / K ** 0.5).bfloat16()
                 bias = torch.randn(N, device="cuda", generator=gen)
-                run = lambda: ops.conv3x3(x, w, bias)
-            bn, _ = launch_info(run)
-            ms = []
-            for _ in range(args.rounds):
-                t, clk = time_it(run)
-                ms.append(t)
-                clocks += [clk] if clk else []
-            med = sorted(ms)[len(ms) // 2]
-            for k in tot:
-                tot[k] += med * cnt
-            row = dict(kind=kind, M=M, N=N, K=K, launches=cnt, sched="cooperative only", old_bn=bn, old_ms=med,
-                       old_spread=(max(ms) - min(ms)) / med, old_tflops=fl / med / 1e9, old_bpf=bpf(bn))
-            print(f"{kind:12s} {M:7d} {N:6d} {K:6d} | coop bn {bn:3d} {med:8.4f} ms {row['old_tflops']:6.1f} TFLOP/s "
-                  f"{bpf(bn):.4f} B/FLOP | (one schedule)", flush=True)
-            rows.append(row)
-            continue
-        geglu = "geglu" in kind
-        a = torch.randn(M, K, device="cuda", generator=gen).bfloat16()
-        w = (torch.randn(N, K, device="cuda", generator=gen) / K ** 0.5).bfloat16()
-        bias = torch.randn(N, device="cuda", generator=gen)
-        res = torch.randn(M, N, device="cuda", generator=gen).bfloat16() if kind in RESIDUAL else None
-        arms = {}
+                res = torch.randn(M, N, device="cuda", generator=gen).bfloat16()   # conv2 of a resnet adds the shortcut
+                make = lambda bn: (lambda: ops.conv3x3(x, w, bias, residual=res, block_n=bn))
+        else:
+            a = torch.randn(M, K, device="cuda", generator=gen).bfloat16()
+            w = (torch.randn(N, K, device="cuda", generator=gen) / K ** 0.5).bfloat16()
+            bias = torch.randn(N, device="cuda", generator=gen)
+            res = torch.randn(M, N, device="cuda", generator=gen).bfloat16() if kind in RESIDUAL else None
 
-        def arm(pp, bn=0):
-            if geglu:
-                gbn = bn or (64 if pp == 1 else ops.geglu_block_n(N))
-                wp, bp, _ = ops.pack_geglu(w, bias, gbn)
-                return lambda: ops.gemm(a, wp, bp, geglu=True, block_n=gbn)
-            return lambda: ops.gemm(a, w, bias, residual=res, block_n=bn)
-        for name, pp in (("old", 0), ("new", 1), ("default", None)):
+            def make(bn, pack=None):
+                if geglu:
+                    wp, bp, _ = ops.pack_geglu(w, bias, pack or bn)
+                    return lambda: ops.gemm(a, wp, bp, geglu=True, block_n=pack or bn)
+                return lambda: ops.gemm(a, w, bias, residual=res, block_n=bn)
+        # arm -> (run, env VX_GEMM_PP, library)
+        arms = {}
+        if baseline is not None:
+            arms["parent"] = (make(256) if geglu else make(0), None, baseline)
+        arms["coop"] = (make(256) if geglu else make(0), 0, lib)
+        for bn in widths:
+            if N % bn == 0 and (not geglu or bn % 64 == 0):
+                arms[f"pp{bn}"] = (make(bn), 1, lib)
+        arms["default"] = (make(0, ops.geglu_block_n(N)) if geglu else make(0), None, lib)
+
+        def use(name):
+            _, pp, l = arms[name]
+            _ffi._lib = l
             set_env(VX_GEMM_PP=pp)
-            run = arm(pp)
-            arms[name] = (run, launch_info(run), pp)
-        nbn = arms["new"][1][0]
-        set_env(VX_GEMM_PP=0)
-        run = arm(0, nbn)
-        arms["same"] = (run, launch_info(run), 0)
-        outs = {}
-        for name, (run, _, pp) in arms.items():
-            set_env(VX_GEMM_PP=pp)
-            outs[name] = run()
+        info, outs = {}, {}
+        for name in arms:
+            use(name)
+            info[name] = launch_info(arms[name][0])
+            outs[name] = arms[name][0]().clone()
         torch.cuda.synchronize()
-        same = all(torch.equal(outs["old"], o) for o in outs.values())
-        timed = ("old", "new", "same")
+        same = all(torch.equal(outs["coop"], o) for o in outs.values())
+        twin = next((k for k in arms if k not in ("default", "parent") and info[k] == info["default"]), None)
+        timed = [k for k in arms if k != "default" or twin is None]
         ms = {k: [] for k in timed}
         for _ in range(args.rounds):
             for name in timed:
-                run, _, pp = arms[name]
-                set_env(VX_GEMM_PP=pp)
-                t, clk = time_it(run)
+                use(name)
+                t, clk = time_it(arms[name][0])
                 ms[name].append(t)
                 clocks += [clk] if clk else []
+        _ffi._lib = lib
         set_env(VX_GEMM_PP=None)
         med = {k: sorted(v)[len(v) // 2] for k, v in ms.items()}
         sp = {k: (max(v) - min(v)) / med[k] for k, v in ms.items()}
-        (obn, _), (nbn, npp), (dbn, dpp), (sbn, spp) = (arms[k][1] for k in ("old", "new", "default", "same"))
-        dflt = "new" if dpp else "same" if dbn == sbn and dbn != obn else "old"
-        tot["old"] += med["old"] * cnt
-        tot["new"] += med["new"] * cnt
-        tot["default"] += med[dflt] * cnt
-        row = dict(kind=kind, M=M, N=N, K=K, launches=cnt, geglu=geglu, bit_equal=same, old_bn=obn, new_bn=nbn,
-                   new_is_pp=bool(npp), same_bn=sbn, default_bn=dbn, default_pp=bool(dpp),
-                   **{f"{k}_ms": med[k] for k in timed}, **{f"{k}_spread": sp[k] for k in timed},
-                   **{f"{k}_tflops": fl / med[k] / 1e9 for k in timed}, old_bpf=bpf(obn), new_bpf=bpf(nbn),
-                   old_over_new=med["old"] / med["new"], same_over_new=med["same"] / med["new"])
-        print(f"{kind:12s} {M:7d} {N:6d} {K:6d} | coop bn {obn:3d} {med['old']:8.4f} ms (+-{100 * sp['old']:4.1f}%) "
-              f"{row['old_tflops']:6.1f} TFLOP/s {bpf(obn):.4f} B/FLOP | pp bn {nbn:3d}{'' if npp else ' (coop)'} "
-              f"{med['new']:8.4f} ms (+-{100 * sp['new']:4.1f}%) {row['new_tflops']:6.1f} TFLOP/s {bpf(nbn):.4f} B/FLOP | "
-              f"coop bn {sbn:3d} {med['same']:8.4f} ms (+-{100 * sp['same']:4.1f}%) | old/new {row['old_over_new']:.3f} "
-              f"same/new {row['same_over_new']:.3f} | default {'pp' if dpp else 'coop'} bn {dbn} | bit-equal {same}",
-              flush=True)
+        if twin is not None:
+            med["default"], sp["default"] = med[twin], sp[twin]
+        fastest = min((k for k in med if k not in ("default", "parent")), key=med.get)
+        tot["coop"] += med["coop"] * cnt
+        tot["default"] += med["default"] * cnt
+        tot["best"] += med[fastest] * cnt
+        tot["parent"] += med.get("parent", 0.0) * cnt
+        row = dict(kind=kind, M=M, N=N, K=K, launches=cnt, geglu=geglu, bit_equal=same, fastest=fastest,
+                   default_is=twin or "default",
+                   arms={k: dict(bn=info[k][0], pp=info[k][1], rr=info[k][2], ms=med[k], spread=sp[k],
+                                 tflops=fl / med[k] / 1e9, bpf=bpf(info[k][0])) for k in med})
+        cells = " | ".join(f"{k} bn {info[k][0]}{'pp' if info[k][1] else 'co'}{'r' if info[k][2] else ''} {med[k]:.4f} ms "
+                           f"(+-{100 * sp[k]:.1f}%) {fl / med[k] / 1e12:.0f}T" for k in med if k != "default")
+        print(f"{kind:12s} {M:7d} {N:6d} {K:6d} | {cells} | default = {twin or 'own'} {med['default']:.4f} ms "
+              f"coop/default {med['coop'] / med['default']:.3f} | fastest {fastest} | bit-equal {same}", flush=True)
         rows.append(row)
     mhz = sorted(clocks)[len(clocks) // 2] if clocks else None
-    print(f"one forward, GEMM + conv launches: cooperative {tot['old']:.2f} ms ({total / tot['old'] / 1e9:.0f} TFLOP/s), "
-          f"ping-pong where available {tot['new']:.2f} ms ({total / tot['new'] / 1e9:.0f} TFLOP/s), "
-          f"default rule {tot['default']:.2f} ms ({total / tot['default'] / 1e9:.0f} TFLOP/s); SM clock {mhz} MHz; {device}")
+    rate = lambda t: f"{t:.2f} ms ({total / t / 1e9:.0f} TFLOP/s)" if t else "not run"
+    print(f"one forward, GEMM + conv launches: parent {rate(tot['parent'])}, cooperative {rate(tot['coop'])}, "
+          f"default rule {rate(tot['default'])}, fastest arm per shape {rate(tot['best'])}; SM clock {mhz} MHz; {device}")
     if args.json:
         with open(args.json, "w") as f:
             json.dump({"device": device, "sm_mhz": mhz, "totals_ms": tot, "rows": rows}, f, indent=1)

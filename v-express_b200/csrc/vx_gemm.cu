@@ -18,13 +18,16 @@
 // Roles (384 threads = three warpgroups): warp 0 = TMA producer, warp 1 = TMA store + residual prefetch;
 // warpgroups 1 and 2 = MMA + epilogue.  Two consumer schedules:
 //   * cooperative: both warpgroups take 64 rows of every 128-row tile (wgmma m64nBNk16, BN <= 256);
-//   * ping-pong (PP, plain GEMM only, BN <= 96): warpgroup w owns the whole 128 x BN tile of every item it = w mod 2 of
-//     the CTA (two m64nBNk16 per K step).  An order barrier hands the tensor pipe over at mainloop boundaries, so one
-//     warpgroup's epilogue runs under the other's MMAs instead of stalling the pipe.
+//   * ping-pong (PP, BN <= 160; plain GEMM and every convolution producer, not the LayerNorm / row-sum variants): warpgroup
+//     w owns the whole 128 x BN tile of every item it = w mod 2 of the CTA (two m64nBNk16 per K step).  An order barrier
+//     hands the tensor pipe over at mainloop boundaries, so one warpgroup's epilogue runs under the other's MMAs instead of
+//     stalling the pipe.
 //   wgmma -> bias/scale (+ residual read from a TMA-prefetched, 64B-swizzled smem tile) -> bf16 -> same smem
 //   tile -> TMA store (coalesced, clipped at the M/N edges by the tensor map).  While the consumers run their
 // epilogue, the producer already fills the ring with the next tile's operands.  Both schedules add the same products in
 // the same K order and round at the same points: their outputs are bit-identical.
+// setmaxnreg moves registers from the producer warpgroup (40 per thread) to the consumers (232): room for 2 x 80 fp32
+// accumulators per thread at ping-pong BN 160.
 #include "vx_host.h"
 #include "vx_ptx.cuh"
 
@@ -34,7 +37,7 @@ constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 constexpr int kThreads = 384;
 constexpr int kEpiThreads = 256;
-constexpr int kPPMaxBN = 96;   // ping-pong: BN accumulators per thread; 128 spills at the 168 registers of 384 threads
+constexpr int kPPMaxBN = 160;  // ping-pong: 2 x BN / 2 accumulators per thread; BN 192 spills at the consumers' 232 registers
 constexpr int kPanelCols = 32;                         // staging panel: 32 bf16 = 64 B rows, 64B swizzle
 constexpr int kPanelBytes = kBlockM * kPanelCols * 2;  // 8 KB
 constexpr int kSmemCap = 227 * 1024;
@@ -210,144 +213,147 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
   // barrier init and the tensor-map prefetch overlapped the previous grid's tail; from here on every role touches global memory
   pdl_wait();
 
-  if (warp < 4) setmaxnreg_dec<40>();   // producer / store warpgroup: few registers, the consumers get the rest
-  else setmaxnreg_inc<232>();
-
-  if (warp == 0) {
-    // ---------------------------------------------------------- TMA producer
-    // The whole warp runs the loop in lock-step so that tile / coordinate / barrier values stay warp-uniform; only the
-    // elected lane issues.
-    const bool leader = elect_one();
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int it = 0, t = item_at(0); t >= 0; t = item_at(++it)) {
-      const int par = t / tiles_per_par, tt = t - par * tiles_per_par;
-      const int tile_n = tt % p.tiles_n, tile_m = tt / p.tiles_n;
-      int n0 = 0, y0 = 0, x0 = 0;
-      const long long m0 = (long long)tile_m * p.rows_valid;
-      if (p.taps != 1) {
-        const long long hw = (long long)p.H * p.W;
-        n0 = (int)(m0 / hw);
-        const int rem = (int)(m0 % hw);
-        y0 = rem / p.W;
-        x0 = rem % p.W;
-      }
-      const uint32_t tx_bytes = (uint32_t)((p.rr ? a_bytes : p.rows_valid * kBlockK * 2) + nbt * b_bytes);
-      const int b_row = par * p.N + tile_n * BN;
-      if constexpr (LNF) {
-        if (p.ares && tile_n == 0) {
-          // resident A: every K block of this row tile is loaded once, in front of the first column tile, into its own
-          // slot -- all of them before any W stage, since the consumers take the row statistics before their first MMA
-          for (int kb = 0; kb < p.kblocks1; ++kb) {
-            mbar_wait(&a_empty[kb], (uint32_t)(((it / p.tiles_n) & 1) ^ 1));
-            if (leader) {
-              mbar_expect_tx(&a_land[kb], (uint32_t)(kBlockM * kBlockK * 2));
-              tma_load_2d(smem + kb * (kBlockM * kBlockK * 2), &mapA, &a_land[kb], kb * kBlockK, (int)m0);
+  // setmaxnreg is .sync.aligned per warpgroup: each one sits at the top of its warpgroup's branch, so that ptxas can give the
+  // consumer code after it the raised budget (issued before the role branches, it is dropped: C7507).
+  if (warp < 4) {
+    setmaxnreg_dec<40>();   // producer / store warpgroup, idle warps 2 and 3 included: few registers
+    if (warp == 0) {
+      // ---------------------------------------------------------- TMA producer
+      // The whole warp runs the loop in lock-step so that tile / coordinate / barrier values stay warp-uniform; only the
+      // elected lane issues.
+      const bool leader = elect_one();
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int it = 0, t = item_at(0); t >= 0; t = item_at(++it)) {
+        const int par = t / tiles_per_par, tt = t - par * tiles_per_par;
+        const int tile_n = tt % p.tiles_n, tile_m = tt / p.tiles_n;
+        int n0 = 0, y0 = 0, x0 = 0;
+        const long long m0 = (long long)tile_m * p.rows_valid;
+        if (p.taps != 1) {
+          const long long hw = (long long)p.H * p.W;
+          n0 = (int)(m0 / hw);
+          const int rem = (int)(m0 % hw);
+          y0 = rem / p.W;
+          x0 = rem % p.W;
+        }
+        const uint32_t tx_bytes = (uint32_t)((p.rr ? a_bytes : p.rows_valid * kBlockK * 2) + nbt * b_bytes);
+        const int b_row = par * p.N + tile_n * BN;
+        if constexpr (LNF) {
+          if (p.ares && tile_n == 0) {
+            // resident A: every K block of this row tile is loaded once, in front of the first column tile, into its own
+            // slot -- all of them before any W stage, since the consumers take the row statistics before their first MMA
+            for (int kb = 0; kb < p.kblocks1; ++kb) {
+              mbar_wait(&a_empty[kb], (uint32_t)(((it / p.tiles_n) & 1) ^ 1));
+              if (leader) {
+                mbar_expect_tx(&a_land[kb], (uint32_t)(kBlockM * kBlockK * 2));
+                tma_load_2d(smem + kb * (kBlockM * kBlockK * 2), &mapA, &a_land[kb], kb * kBlockK, (int)m0);
+              }
+            }
+            __syncwarp();
+          }
+        }
+        for (int kb = 0; kb < total_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = ring + stage * stage_bytes;
+          uint8_t* sb = sa + a_bytes;
+          const int tap = p.taps != 1 ? kb / p.kblocks1 : 0;     // rr: tap = dx index (0..2)
+          const int cb = kb - tap * p.kblocks1;
+          if constexpr (LNF) {
+            if (p.ares) {
+              if (leader) {
+                mbar_expect_tx(&full_bar[stage], (uint32_t)b_bytes);
+                tma_load_2d(ring + stage * stage_bytes, &mapB, &full_bar[stage], kb * kBlockK, b_row);
+              }
+              __syncwarp();
+              if (++stage == p.stages) {
+                stage = 0;
+                phase ^= 1;
+              }
+              continue;
+            }
+          }
+          if (leader) {
+            mbar_expect_tx(&full_bar[stage], tx_bytes);
+            if (p.rr) {
+              // A: image rows y0 - 1 .. y0 + hbox of the column window shifted by dx (zero-filled outside the image =
+              // padding); W: the three taps (dy, dx), dy = 0..2, of this channel block
+              tma_load_4d(sa, &mapA, &full_bar[stage], cb * kBlockK, x0 + tap - 1, y0 - 1, n0);
+  #pragma unroll
+              for (int dyi = 0; dyi < 3; ++dyi)
+                tma_load_2d(sb + dyi * b_bytes, &mapB, &full_bar[stage], ((dyi * 3 + tap) * p.kblocks1 + cb) * kBlockK, b_row);
+            } else {
+              // 3x3: taps (dy, dx) in {-1, 0, 1}^2.  Folded upsample: output pixel (2i + py, 2j + px) reads the 2x2 input
+              // neighbourhood rows i + py - 1 + {0, 1}, columns j + px - 1 + {0, 1} (weights pre-summed per parity on the host).
+              const int dy = p.ups ? (tap >> 1) + (par >> 1) - 1 : tap / 3 - p.cpad;
+              const int dx = p.ups ? (tap & 1) + (par & 1) - 1 : tap % 3 - p.cpad;
+              if (p.taps != 1) {
+                tma_load_4d(sa, &mapA, &full_bar[stage], cb * kBlockK, x0 * p.cstride + dx, y0 * p.cstride + dy, n0);
+              } else if (kb < p.kblocks1) {
+                tma_load_2d(sa, &mapA, &full_bar[stage], kb * kBlockK, (int)m0);
+              } else {
+                tma_load_2d(sa, &mapA2, &full_bar[stage], (kb - p.kblocks1) * kBlockK, (int)m0);
+              }
+              tma_load_2d(sb, &mapB, &full_bar[stage], kb * kBlockK, b_row);
             }
           }
           __syncwarp();
-        }
-      }
-      for (int kb = 0; kb < total_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = ring + stage * stage_bytes;
-        uint8_t* sb = sa + a_bytes;
-        const int tap = p.taps != 1 ? kb / p.kblocks1 : 0;     // rr: tap = dx index (0..2)
-        const int cb = kb - tap * p.kblocks1;
-        if constexpr (LNF) {
-          if (p.ares) {
-            if (leader) {
-              mbar_expect_tx(&full_bar[stage], (uint32_t)b_bytes);
-              tma_load_2d(ring + stage * stage_bytes, &mapB, &full_bar[stage], kb * kBlockK, b_row);
-            }
-            __syncwarp();
-            if (++stage == p.stages) {
-              stage = 0;
-              phase ^= 1;
-            }
-            continue;
+          if (++stage == p.stages) {
+            stage = 0;
+            phase ^= 1;
           }
         }
-        if (leader) {
-          mbar_expect_tx(&full_bar[stage], tx_bytes);
-          if (p.rr) {
-            // A: image rows y0 - 1 .. y0 + hbox of the column window shifted by dx (zero-filled outside the image =
-            // padding); W: the three taps (dy, dx), dy = 0..2, of this channel block
-            tma_load_4d(sa, &mapA, &full_bar[stage], cb * kBlockK, x0 + tap - 1, y0 - 1, n0);
-#pragma unroll
-            for (int dyi = 0; dyi < 3; ++dyi)
-              tma_load_2d(sb + dyi * b_bytes, &mapB, &full_bar[stage], ((dyi * 3 + tap) * p.kblocks1 + cb) * kBlockK, b_row);
-          } else {
-            // 3x3: taps (dy, dx) in {-1, 0, 1}^2.  Folded upsample: output pixel (2i + py, 2j + px) reads the 2x2 input
-            // neighbourhood rows i + py - 1 + {0, 1}, columns j + px - 1 + {0, 1} (weights pre-summed per parity on the host).
-            const int dy = p.ups ? (tap >> 1) + (par >> 1) - 1 : tap / 3 - p.cpad;
-            const int dx = p.ups ? (tap & 1) + (par & 1) - 1 : tap % 3 - p.cpad;
-            if (p.taps != 1) {
-              tma_load_4d(sa, &mapA, &full_bar[stage], cb * kBlockK, x0 * p.cstride + dx, y0 * p.cstride + dy, n0);
-            } else if (kb < p.kblocks1) {
-              tma_load_2d(sa, &mapA, &full_bar[stage], kb * kBlockK, (int)m0);
-            } else {
-              tma_load_2d(sa, &mapA2, &full_bar[stage], (kb - p.kblocks1) * kBlockK, (int)m0);
-            }
-            tma_load_2d(sb, &mapB, &full_bar[stage], kb * kBlockK, b_row);
-          }
-        }
-        __syncwarp();
-        if (++stage == p.stages) {
-          stage = 0;
-          phase ^= 1;
-        }
       }
-    }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------- TMA store + residual prefetch (one lane)
-    if (lane == 0 && !p.out_f32) {
-      const uint32_t res_bytes = (uint32_t)(p.rows_valid * out_cols * 2);
-      auto arm = [&](int t, int b) {  // make staging tile b usable for output tile t
-        if (p.has_residual) {   // (never with ups: the upsampler convs have no residual)
-          const int tn_ = t % p.tiles_n, tm_ = t / p.tiles_n;
-          mbar_expect_tx(&c_ready[b], res_bytes);
-          for (int pn = 0; pn < npanels; ++pn)
-            tma_load_2d(sC + b * buf_bytes + pn * kPanelBytes, &mapR, &c_ready[b], tn_ * out_cols + pn * kPanelCols,
-                        tm_ * p.rows_valid);
-        } else {
-          mbar_arrive(&c_ready[b]);
-        }
-      };
-      for (int b = 0; b < p.nbuf; ++b)
-        if (item_at(b) >= 0) arm(item_at(b), b);
-      for (int it = 0, t = item_at(0); t >= 0; t = item_at(++it)) {
-        const int b = it % p.nbuf;
-        const int par = t / tiles_per_par, tt = t - par * tiles_per_par;
-        const int tile_n = tt % p.tiles_n, tile_m = tt / p.tiles_n;
-        mbar_wait(&staged[b], (uint32_t)((it / p.nbuf) & 1));
-        if (p.ups) {
-          // rows of the tile = low-resolution pixels (n, i, j); they land on (n, 2i + py, 2j + px): 5-D map (c, j, i, n, py)
-          // per px (mapC: px = 0, mapR: px = 1)
-          const long long m0 = (long long)tile_m * p.rows_valid, hw = (long long)p.H * p.W;
-          const int n0 = (int)(m0 / hw), rem = (int)(m0 % hw);
-          const CUtensorMap* mo = (par & 1) ? &mapR : &mapC;
-          if (m0 < p.M)
+    } else if (warp == 1) {
+      // ---------------------------------------------------------- TMA store + residual prefetch (one lane)
+      if (lane == 0 && !p.out_f32) {
+        const uint32_t res_bytes = (uint32_t)(p.rows_valid * out_cols * 2);
+        auto arm = [&](int t, int b) {  // make staging tile b usable for output tile t
+          if (p.has_residual) {   // (never with ups: the upsampler convs have no residual)
+            const int tn_ = t % p.tiles_n, tm_ = t / p.tiles_n;
+            mbar_expect_tx(&c_ready[b], res_bytes);
             for (int pn = 0; pn < npanels; ++pn)
-              tma_store_5d(mo, sC + b * buf_bytes + pn * kPanelBytes, tile_n * out_cols + pn * kPanelCols, rem % p.W,
-                           rem / p.W, n0, par >> 1);
-        } else {
-          for (int pn = 0; pn < npanels; ++pn)
-            tma_store_2d(&mapC, sC + b * buf_bytes + pn * kPanelBytes, tile_n * out_cols + pn * kPanelCols,
-                         tile_m * p.rows_valid);
+              tma_load_2d(sC + b * buf_bytes + pn * kPanelBytes, &mapR, &c_ready[b], tn_ * out_cols + pn * kPanelCols,
+                          tm_ * p.rows_valid);
+          } else {
+            mbar_arrive(&c_ready[b]);
+          }
+        };
+        for (int b = 0; b < p.nbuf; ++b)
+          if (item_at(b) >= 0) arm(item_at(b), b);
+        for (int it = 0, t = item_at(0); t >= 0; t = item_at(++it)) {
+          const int b = it % p.nbuf;
+          const int par = t / tiles_per_par, tt = t - par * tiles_per_par;
+          const int tile_n = tt % p.tiles_n, tile_m = tt / p.tiles_n;
+          mbar_wait(&staged[b], (uint32_t)((it / p.nbuf) & 1));
+          if (p.ups) {
+            // rows of the tile = low-resolution pixels (n, i, j); they land on (n, 2i + py, 2j + px): 5-D map (c, j, i, n, py)
+            // per px (mapC: px = 0, mapR: px = 1)
+            const long long m0 = (long long)tile_m * p.rows_valid, hw = (long long)p.H * p.W;
+            const int n0 = (int)(m0 / hw), rem = (int)(m0 % hw);
+            const CUtensorMap* mo = (par & 1) ? &mapR : &mapC;
+            if (m0 < p.M)
+              for (int pn = 0; pn < npanels; ++pn)
+                tma_store_5d(mo, sC + b * buf_bytes + pn * kPanelBytes, tile_n * out_cols + pn * kPanelCols, rem % p.W,
+                             rem / p.W, n0, par >> 1);
+          } else {
+            for (int pn = 0; pn < npanels; ++pn)
+              tma_store_2d(&mapC, sC + b * buf_bytes + pn * kPanelBytes, tile_n * out_cols + pn * kPanelCols,
+                           tile_m * p.rows_valid);
+          }
+          tma_store_commit();
+          const int tnext = item_at(it + p.nbuf);
+          if (tnext >= 0) {
+            tma_store_wait_read();  // the store has finished reading tile b
+            arm(tnext, b);
+          }
         }
-        tma_store_commit();
-        const int tnext = item_at(it + p.nbuf);
-        if (tnext >= 0) {
-          tma_store_wait_read();  // the store has finished reading tile b
-          arm(tnext, b);
-        }
+        tma_store_wait_all();
       }
-      tma_store_wait_all();
     }
-  } else if (warp >= 4) {
+  } else {
+    setmaxnreg_inc<232>();   // consumer warpgroups: the registers the producer warpgroup gave up
     // -------------------------------------------------------------- MMA + epilogue (warpgroups 1, 2)
-    static_assert(!(PP && LNF) && (!PP || BN <= kPPMaxBN), "ping-pong: plain epilogues, BN <= 96");
+    static_assert(!(PP && LNF) && (!PP || BN <= kPPMaxBN), "ping-pong: plain epilogues, BN <= 160");
     constexpr int MH = PP ? 2 : 1;                  // 64-row accumulator blocks per warpgroup
     const int wg = (threadIdx.x >> 7) - 1;          // cooperative: rows [64 wg, 64 wg + 64) of the tile; PP: items wg mod 2
     const int wrow = (PP ? 0 : wg * 64) + (warp & 3) * 16 + (lane >> 2);   // + 8 h (+ 64 mh): the rows of this thread
@@ -436,16 +442,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
         }
         if constexpr (!PP) sa += (uint32_t)(wg * 64 * 128);
         wgmma_fence();
-        if (!PP && p.rr) {
+        if (p.rr) {
           // tap dy reads the 128 tile rows that start dy image rows (W x 128 B, a multiple of the 1024-B swizzle atom)
           // into the A box, against its own W tile
 #pragma unroll
           for (int dyi = 0; dyi < 3; ++dyi) {
-            const uint64_t da = make_smem_desc(sa + (uint32_t)(dyi * p.W * 128), 16, 1024, SWZ_128B);
             const uint64_t db = make_smem_desc(sb + (uint32_t)(dyi * b_bytes), 16, 1024, SWZ_128B);
 #pragma unroll
             for (int k = 0; k < kBlockK / 16; ++k)   // +32 bytes per K step = +2 in the (addr >> 4) field
-              Wgmma<BN>::template ss<0, 0>(acc[0], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | dyi | k) != 0);
+#pragma unroll
+              for (int mh = 0; mh < MH; ++mh) {
+                const uint64_t da = make_smem_desc(sa + (uint32_t)(dyi * p.W * 128 + mh * 64 * 128), 16, 1024, SWZ_128B);
+                Wgmma<BN>::template ss<0, 0>(acc[mh], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | dyi | k) != 0);
+              }
           }
         } else {
           const uint64_t db = make_smem_desc(sb, 16, 1024, SWZ_128B);
@@ -640,45 +649,60 @@ static bool bn_supported(int bn) {
 }
 
 // column-tile widths the ping-pong schedule is instantiated for
-static bool pp_bn_supported(int bn) { return bn == 32 || bn == 64 || bn == 96; }
+static bool pp_bn_supported(int bn) { return bn == 32 || bn == 64 || bn == 96 || bn == 128 || bn == 160; }
 
-// Pick the schedule and the wgmma N (only `fixed_bn` if it is set).
-// Ping-pong (where `pp_ok`): the widest ping-pong width that divides N and is a multiple of `gran`.  By default only bn 96.
-//   Measured with tools/gemm_ab.py (H100 SXM, DESIGN section 9): at the same 128 x bn tile, ping-pong is x1.05 to x1.23 faster
-//   than cooperative on every plain-GEMM shape of the benchmark forward, so the schedule pays wherever it runs.  Against the
-//   wider cooperative tile the cost model below picks, only bn 96 wins (the qkv projections, N = 3 C: x1.03 to x1.19).  Bn 64
-//   moves more operand bytes per FLOP from L2 and loses to the cooperative bn 160 / 256 tile on every shape with M >= 8192
-//   (x0.79 to x0.99).  VX_GEMM_PP=1 allows bn 64 / 32 too.
-// Cooperative: among the supported widths (multiples of `gran` that divide N), minimise waves(tiles) x (cycles per K
-//   block x K blocks + epilogue).  Cycles per 128 x bn x 64 block = max(MMA 4 bn, shared-memory operand feed 128 + 2 bn at
-//   128 B/clk: A once, W once per consumer warpgroup) + issue overhead.
-// VX_GEMM_PP=0 never picks ping-pong.
+// Same-tile speed-up of the ping-pong schedule over the cooperative one on a CTA that walks two tiles or more (the
+// epilogue and the tile-boundary drain of one warpgroup run under the other's MMAs), and the longest K loop (in 64-wide
+// blocks) it pays on: beyond K = 1280 one warpgroup's mainloop, which waits on its own MMAs every stage, feeds the tensor
+// pipe worse than two cooperative ones and the hidden epilogue no longer makes up for it.  Row-reuse convolutions are
+// exempt (their ping-pong ring is deeper than the cooperative one).  Measured with tools/gemm_ab.py (DESIGN section 9).
+constexpr double kPPGain = 1.12;
+constexpr int kPPMaxKBlocks = 20;
+
+// Pick the schedule and the wgmma N (only `fixed_bn` if it is set).  Among the supported widths (multiples of `gran` that
+// divide N) and both schedules, minimise waves(tiles) x tile cost, waves = tiles per CTA of the persistent grid.
+//   Cooperative tile: cycles per K block x K blocks + epilogue, cycles per 128 x bn x 64 block = max(MMA 4 bn,
+//   shared-memory operand feed 128 + 2 bn at 128 B/clk: A once, W once per consumer warpgroup) + issue overhead.
+//   Ping-pong (where `pp_ok`, bn <= pp_max_bn and, unless `pp_any_k`, total_kb <= kPPMaxKBlocks): the same tile cost /
+//   kPPGain when a CTA gets two tiles or more.  With one tile per CTA (small M) there is no second tile to overlap and one
+//   warpgroup would idle: the cooperative schedule.
+// Ties go to the wider tile, then to the cooperative schedule.
+// VX_GEMM_PP=0: cooperative only (the widths are the cost model's); 1: ping-pong at the widest width that divides N.
 static int pick_block_n(long long tiles_m, int N, int gran, int total_kb, int fixed_bn = 0, bool pp_ok = false,
-                        int* pp = nullptr) {
+                        int* pp = nullptr, int pp_max_bn = kPPMaxBN, bool pp_any_k = false) {
   const int mode = gemm_env().pp;
+  auto fits = [&](int bn) { return N % bn == 0 && bn % gran == 0 && bn_supported(bn) && (fixed_bn <= 0 || bn == fixed_bn); };
   if (pp) *pp = 0;
-  if (pp_ok && mode != 0) {
-    for (int bn = kPPMaxBN; bn >= 32; bn -= 32) {
-      if (mode == -1 && bn != kPPMaxBN) break;
-      if (N % bn || bn % gran || (fixed_bn > 0 && bn != fixed_bn)) continue;
-      if (pp) *pp = 1;
-      return bn;
-    }
+  pp_ok = pp_ok && pp && mode != 0;
+  if (pp_ok && mode == 1) {
+    for (int bn = kPPMaxBN; bn >= 32; bn -= 32)
+      if (fits(bn) && pp_bn_supported(bn) && bn <= pp_max_bn) {
+        *pp = 1;
+        return bn;
+      }
   }
+  if (!pp_any_k && total_kb > kPPMaxKBlocks) pp_ok = false;
   const int sms = device_sms();
-  int best = 0;
+  int best = 0, best_pp = 0;
   double best_cost = 1e30;
   for (int bn = 256; bn >= gran; bn -= gran) {
-    if (N % bn || !bn_supported(bn) || (fixed_bn > 0 && bn != fixed_bn)) continue;
+    if (!fits(bn)) continue;
     const long long items = tiles_m * (N / bn);
-    const double waves = (double)((items + sms - 1) / sms);
+    const long long waves = (items + sms - 1) / sms;
     const double cyc = (4.0 * bn > 128.0 + 2.0 * bn) ? 4.0 * bn : 128.0 + 2.0 * bn;
-    const double cost = waves * (total_kb * (cyc + 40.0) + 4.0 * bn);
+    const double cost = (double)waves * (total_kb * (cyc + 40.0) + 4.0 * bn);
     if (cost < best_cost * 0.999) {
       best_cost = cost;
       best = bn;
+      best_pp = 0;
+    }
+    if (pp_ok && pp_bn_supported(bn) && bn <= pp_max_bn && waves >= 2 && cost / kPPGain < best_cost * 0.999) {
+      best_cost = cost / kPPGain;
+      best = bn;
+      best_pp = 1;
     }
   }
+  if (pp) *pp = best_pp;
   return best;
 }
 
@@ -703,6 +727,8 @@ static cudaError_t launch_lnf(const CUtensorMap& mA, const CUtensorMap& mA2, con
         case 32: return launch_bn<32, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
         case 64: return launch_bn<64, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
         case 96: return launch_bn<96, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        case 128: return launch_bn<128, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        case 160: return launch_bn<160, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
         default: return cudaErrorInvalidValue;
       }
     }
@@ -736,10 +762,10 @@ static int launch(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorM
   int nbuf = (!a.out_f32 && (size_t)3 * stage_bytes + 2 * buf_bytes <= cap) ? 2 : 1;
   if (a.rr) {
     // a row-reuse stage is 3 taps deep (12 MMAs per warpgroup): three stages when they fit beside ONE staging tile, else
-    // two beside two
-    nbuf = ((size_t)3 * stage_bytes + buf_bytes <= cap) ? 1 : 2;
-    want_stages = nbuf == 1 ? 3 : 2;
-    if ((size_t)want_stages * stage_bytes + (size_t)nbuf * buf_bytes > cap) nbuf = 1;
+    // two beside two.  Ping-pong: three stages beside two staging tiles (conv3x3_entry checked that they fit)
+    nbuf = (a.pp || (size_t)3 * stage_bytes + buf_bytes > cap) ? 2 : 1;
+    want_stages = nbuf == 1 || a.pp ? 3 : 2;
+    if (!a.pp && (size_t)want_stages * stage_bytes + (size_t)nbuf * buf_bytes > cap) nbuf = 1;
   }
   if (a.ares) {   // every column tile of a row tile streams the whole W panel: a deep ring, two staging tiles when they fit
     nbuf = ((size_t)4 * stage_bytes + 2 * (size_t)buf_bytes <= cap) ? 2 : 1;
@@ -757,12 +783,11 @@ static int launch(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorM
   VX_REQUIRE(smem <= (size_t)kSmemCap, "vx_gemm: %zu bytes of shared memory needed (bn=%d, K blocks=%d)", smem, a.block_n,
              a.kblocks1);
   if (gemm_env().verbose)
-    fprintf(stderr, "[vx_gemm] M=%d N=%d kb=%d taps=%d bn=%d pp=%d stages=%d nbuf=%d tiles=%dx%d\n", a.M, a.N, total_kb,
-            a.taps, a.block_n, a.pp, stages, nbuf, a.tiles_m, a.tiles_n);
+    fprintf(stderr, "[vx_gemm] M=%d N=%d kb=%d taps=%d bn=%d pp=%d rr=%d stages=%d nbuf=%d tiles=%dx%d\n", a.M, a.N,
+            total_kb, a.taps, a.block_n, a.pp, a.rr, stages, nbuf, a.tiles_m, a.tiles_n);
   const int npar = a.ups ? 4 : 1;
   const bool lnf = a.ln_stats != nullptr || a.ln_parts != nullptr || a.ares;
-  VX_REQUIRE(!a.pp || (a.taps == 1 && !lnf && !a.rs_out && pp_bn_supported(a.block_n)), "vx_gemm: no ping-pong kernel for bn=%d",
-             a.block_n);
+  VX_REQUIRE(!a.pp || (!lnf && !a.rs_out && pp_bn_supported(a.block_n)), "vx_gemm: no ping-pong kernel for bn=%d", a.block_n);
   const long long tiles = a.ares ? a.tiles_m : (long long)a.tiles_m * a.tiles_n * npar;
   const int grid = tiles < device_sms() ? (int)tiles : device_sms();
   if (lnf) VX_CHECK_CUDA((launch_lnf<true>(mA, mA2, mB, mR, mC, a, grid, smem, st)));
@@ -1019,18 +1044,31 @@ static int conv3x3_entry(const void* X, int NB, int Hin, int Win, int C, const v
   VX_REQUIRE(M % rows_valid == 0, "vx_conv3x3_bf16: NB*H*W=%lld not tileable by %d", M, rows_valid);
   const long long tiles_m = M / rows_valid;
   const int total_kb = 9 * (C / kBlockK);
-  if (block_n <= 0) block_n = gemm_env().bn;
-  if (block_n <= 0) block_n = pick_block_n(tiles_m, Cout, 32, total_kb);
-  VX_REQUIRE(block_n % 32 == 0 && block_n >= 32 && block_n <= 256 && Cout % block_n == 0,
-             "vx_conv3x3_bf16: block_n=%d invalid for Cout=%d", block_n, Cout);
   // Row reuse: when a tile is hbox >= 2 whole image rows of one frame, ONE box of hbox + 2 rows per (dx, channel block)
   // serves the three dy taps (each tap's 128 rows start dy image rows further down, a multiple of the swizzle atom):
-  // 3 (hbox + 2) / (9 hbox) of the A traffic.
+  // 3 (hbox + 2) / (9 hbox) of the A traffic.  It needs two ring stages beside one staging tile; ping-pong takes it with
+  // three stages beside two staging tiles (one per warpgroup: with two stages it lost to the cooperative schedule at every
+  // shape measured).  Its K order (dx, channel block, dy) differs from tap by tap (dy, dx, channel block), so the producer
+  // is chosen at the cooperative schedule's width, and ping-pong is only taken at widths where the same producer fits: the
+  // result does not depend on the schedule.
   bool rr = gemm_env().conv_rr && stride == 1 && nbox == 1 && wbox == W && hbox >= 2 && rows_valid == kBlockM && (W * 128) % 1024 == 0;
-  if (rr) {   // two ring stages + one staging tile must fit
-    const size_t st = (size_t)(hbox + 2) * W * kBlockK * 2 + (size_t)3 * block_n * kBlockK * 2;
-    if (2 * st + (size_t)(block_n / kPanelCols) * kPanelBytes > (size_t)kSmemCap - kSmemReserve) rr = false;
+  auto rr_fits = [&](int bn, int stages, int nbuf) {
+    const size_t st = (size_t)(hbox + 2) * W * kBlockK * 2 + (size_t)3 * bn * kBlockK * 2;
+    return stages * st + (size_t)nbuf * (bn / kPanelCols) * kPanelBytes <= (size_t)kSmemCap - kSmemReserve;
+  };
+  if (block_n <= 0) block_n = gemm_env().bn;
+  int pp = 0;
+  {
+    const int fixed = block_n;
+    const int coop_bn = pick_block_n(tiles_m, Cout, 32, total_kb, fixed);
+    rr = rr && coop_bn > 0 && rr_fits(coop_bn, 2, 1);
+    int pp_max_bn = kPPMaxBN;
+    while (rr && pp_max_bn > 0 && !rr_fits(pp_max_bn, 3, 2)) pp_max_bn -= 32;
+    block_n = pick_block_n(tiles_m, Cout, 32, total_kb, fixed, true, &pp, pp_max_bn, rr);
+    if (!block_n) block_n = fixed;   // not a width the picker knows: rejected below
   }
+  VX_REQUIRE(block_n % 32 == 0 && block_n >= 32 && block_n <= 256 && Cout % block_n == 0,
+             "vx_conv3x3_bf16: block_n=%d invalid for Cout=%d", block_n, Cout);
   CUtensorMap mA, mB, mR, mC;
   {
     uint64_t dims[4] = {(uint64_t)C, (uint64_t)Win, (uint64_t)Hin, (uint64_t)NB};
@@ -1054,6 +1092,7 @@ static int conv3x3_entry(const void* X, int NB, int Hin, int Win, int C, const v
   a.rr = rr ? 1 : 0;
   a.a_bytes = rr ? (hbox + 2) * W * kBlockK * 2 : kBlockM * kBlockK * 2;
   a.block_n = block_n;
+  a.pp = pp;
   a.rows_valid = rows_valid;
   a.W = W; a.H = H;
   a.cstride = stride; a.cpad = pad_lo;
@@ -1116,7 +1155,12 @@ extern "C" int vx_upconv3x3_bf16(const void* X, int NB, int H, int W, int C, con
   const long long tiles_m = M / rows_valid;
   const int total_kb = 4 * (C / kBlockK);
   if (block_n <= 0) block_n = gemm_env().bn;
-  if (block_n <= 0) block_n = pick_block_n(tiles_m * 4, Cout, 32, total_kb);
+  int pp = 0;
+  {
+    const int fixed = block_n;
+    block_n = pick_block_n(tiles_m * 4, Cout, 32, total_kb, fixed, true, &pp);
+    if (!block_n) block_n = fixed;
+  }
   VX_REQUIRE(block_n % 32 == 0 && block_n >= 32 && block_n <= 256 && Cout % block_n == 0,
              "vx_upconv3x3_bf16: block_n=%d invalid for Cout=%d", block_n, Cout);
   CUtensorMap mA, mB, mC0, mC1;
@@ -1150,6 +1194,7 @@ extern "C" int vx_upconv3x3_bf16(const void* X, int NB, int H, int W, int C, con
   a.ups = 1;
   a.cstride = 1; a.cpad = 1;
   a.block_n = block_n;
+  a.pp = pp;
   a.rows_valid = rows_valid;
   a.W = W; a.H = H;
   a.tiles_m = (int)tiles_m;
