@@ -33,6 +33,18 @@ int vx_gemm_bf16(const void* A, long long lda, int K1, const void* A2, long long
                  const void* residual, long long ldr, void* out, long long ldc, int out_f32, int block_n,
                  void* stream);
 
+/* ---- e4m3 wgmma GEMM (opt-in FP8 mode, UNet3DConditionModel.enable_fp8_linear): A [M, K] and W [N, K] hold
+ * float8_e4m3fn codes (K-major; K, lda, ldw multiples of 16) with one fp32 scale per row of A (a_scale, from
+ * vx_layernorm_fp8) and per output channel of W (w_scale, ops.quantize_fp8_weight).  out = epilogue(a_scale[m] *
+ * w_scale[n] * sum_k A[m,k] W[n,k]) in bf16, the epilogue (bias, bias2, scale, residual; or geglu = 1 with W, w_scale and
+ * bias packed per column tile as for vx_gemm_bf16) as in vx_gemm_bf16.  Replaces the nn.Linear layers fed by an
+ * nn.LayerNorm: the fused attn1 to_q|to_k|to_v, attn1_5.to_q, attn2.to_q and ff.net.0.proj (GEGLU) of the spatial
+ * transformer blocks (modules/attention.py:329-375) and the fused to_q|to_k|to_v and ff.net.0.proj of the motion modules
+ * (modules/motion_module.py:228-234,280-290).  block_n = 0 lets the library choose. */
+int vx_gemm_fp8(const void* A, long long lda, const float* a_scale, int K, const void* W, long long ldw,
+                const float* w_scale, int M, int N, const float* bias, const float* bias2, int bias2_div, float scale,
+                const void* residual, long long ldr, void* out, long long ldc, int geglu, int block_n, void* stream);
+
 /* ---- LayerNorm folded into the consumer GEMM (VX_LN_FOLD=1; run on hardware in round 2: parity green, no gain with the
  * separate statistics pass -- see vx_gemm_rowsums_bf16 for the variant without one).  vx_row_stats writes (mean, rstd) per row of the
  * un-normalised activations; vx_gemm_lnfold_bf16 computes rstd[m] * (A @ Wt^T - mean[m] * colsum) + bias with
@@ -128,6 +140,12 @@ int vx_groupnorm_cluster(const void* x1, long long ld1, int C1, const void* x2, 
 int vx_layernorm(const void* x, long long ldx, long long rows, int C, const float* gamma, const float* beta,
                  float eps, const float* pe, int rows_per_frame, int pe_frames, void* out, long long ldo,
                  void* stream);
+/* vx_layernorm writing the A operand of vx_gemm_fp8: out [rows, ldo] float8_e4m3fn codes sat_rn(y / row_scale[row]) of
+ * the fp32 LayerNorm (+ pe) result y (not rounded through bf16), row_scale[row] = amax(|y|) / 448 (1 for an all-zero
+ * row).  Same call sites as vx_layernorm, for the LayerNorms that feed the GEMMs listed at vx_gemm_fp8. */
+int vx_layernorm_fp8(const void* x, long long ldx, long long rows, int C, const float* gamma, const float* beta,
+                     float eps, const float* pe, int rows_per_frame, int pe_frames, void* out, long long ldo,
+                     float* row_scale, void* stream);
 
 /* ---- GEGLU gate: x [rows, 2*inner] = (h | gate) -> h * gelu_erf(gate) (diffusers GEGLU, SURVEY.md B.3). */
 int vx_geglu(const void* x, long long ldx, long long rows, int inner, void* out, long long ldo, void* stream);

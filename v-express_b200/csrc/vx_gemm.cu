@@ -28,13 +28,23 @@
 // the same K order and round at the same points: their outputs are bit-identical.
 // setmaxnreg moves registers from the producer warpgroup (40 per thread) to the consumers (232): room for 2 x 80 fp32
 // accumulators per thread at ping-pong BN 160.
+//
+// e4m3 operands (TIn = __nv_fp8_e4m3, vx_gemm_fp8; plain producer, linear / GEGLU epilogues, both schedules): a 128-element
+// e4m3 K block is the same 128-byte swizzled row as a 64-element bf16 block, so stages, TMA boxes (UINT8 maps),
+// descriptors and shared-memory budget keep their byte geometry; each stage is four m64nBNk32 e4m3 steps instead of four
+// m64nBNk16 bf16 steps.  The epilogue multiplies the fp32 accumulator by a_scale[m] * w_scale[n] (per-row activation
+// scale, per-output-channel weight scale) before bias / GEGLU / scale / residual.  One accumulator runs over the whole K,
+// as for bf16: the tensor cores add e4m3 products with fewer bits than fp32 (about 14; measured on H100: 2^-14.4 of
+// sum |a_k w_k| at K = 64, 2^-11.3 at K = 1280), which is far below the 2^-4 rounding of the e4m3 operands themselves
+// (tests/test_fp8_gpu.py states the accumulator model its bound assumes; DESIGN section 3 why there is no promotion).
+#include <cuda_fp8.h>
 #include "vx_host.h"
 #include "vx_ptx.cuh"
 
 namespace vx {
 
 constexpr int kBlockM = 128;
-constexpr int kBlockK = 64;
+constexpr int kBlockK = 64;                            // bf16 elements per K block (128 bytes; 128 e4m3 elements)
 constexpr int kThreads = 384;
 constexpr int kEpiThreads = 256;
 constexpr int kPPMaxBN = 160;  // ping-pong: 2 x BN / 2 accumulators per thread; BN 192 spills at the consumers' 232 registers
@@ -90,6 +100,9 @@ struct GemmArgs {
   int ln_nparts;
   float ln_invK;
   float ln_eps;
+  // e4m3 instantiations: out = acc * a_scale[m] * w_scale[n] before the rest of the epilogue (null for bf16)
+  const float* a_scale;   // [M]
+  const float* w_scale;   // [N] (GEGLU: in the packed value|gate column order of W)
 };
 
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
@@ -141,10 +154,17 @@ __device__ __forceinline__ uint32_t* staging_word(uint8_t* buf, int row, int col
   return reinterpret_cast<uint32_t*>(buf + (col >> 5) * kPanelBytes + o);
 }
 
+// One 32-byte K step of both K-major operands (m64nBNk16 bf16 or m64nBNk32 e4m3) from shared memory.
+template <int BN, typename TIn>
+__device__ __forceinline__ void mma_step(float (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
+  if constexpr (sizeof(TIn) == 1) WgmmaE4m3<BN>::ss(d, da, db, scale_d);
+  else Wgmma<BN>::template ss<0, 0>(d, da, db, scale_d);
+}
+
 // wgmma accumulator fragment of m64nBN (per thread): element 4 * g + 2 * h + e sits at row 16 * warp + lane / 4 + 8 * h,
 // column 8 * g + 2 * (lane % 4) + e of the warpgroup's 64 x BN block.  Ping-pong: acc[mh] is the block of rows
-// [64 mh, 64 mh + 64) of the tile.
-template <int BN, bool LNF, bool PP>
+// [64 mh, 64 mh + 64) of the tile.  TIn: operand type (__nv_bfloat16, or __nv_fp8_e4m3 with the scaled epilogue).
+template <int BN, bool LNF, bool PP, typename TIn>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapA2,
                   const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapR,
@@ -152,6 +172,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment required by the 128B swizzle atom
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr bool F8 = sizeof(TIn) == 1;
+  static_assert(!(F8 && LNF), "e4m3: plain producer only");
+  constexpr int KE = kBlockK * 2 / (int)sizeof(TIn);   // elements per 128-byte K block (TMA coordinates)
   const int a_bytes = p.a_bytes;
   constexpr int b_bytes = BN * kBlockK * 2;
   const int nbt = p.rr ? 3 : 1;                         // W tiles per stage (rr: the three dy taps of one dx)
@@ -289,11 +312,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
               if (p.taps != 1) {
                 tma_load_4d(sa, &mapA, &full_bar[stage], cb * kBlockK, x0 * p.cstride + dx, y0 * p.cstride + dy, n0);
               } else if (kb < p.kblocks1) {
-                tma_load_2d(sa, &mapA, &full_bar[stage], kb * kBlockK, (int)m0);
+                tma_load_2d(sa, &mapA, &full_bar[stage], kb * KE, (int)m0);
               } else {
-                tma_load_2d(sa, &mapA2, &full_bar[stage], (kb - p.kblocks1) * kBlockK, (int)m0);
+                tma_load_2d(sa, &mapA2, &full_bar[stage], (kb - p.kblocks1) * KE, (int)m0);
               }
-              tma_load_2d(sb, &mapB, &full_bar[stage], kb * kBlockK, b_row);
+              tma_load_2d(sb, &mapB, &full_bar[stage], kb * KE, b_row);
             }
           }
           __syncwarp();
@@ -453,17 +476,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
 #pragma unroll
               for (int mh = 0; mh < MH; ++mh) {
                 const uint64_t da = make_smem_desc(sa + (uint32_t)(dyi * p.W * 128 + mh * 64 * 128), 16, 1024, SWZ_128B);
-                Wgmma<BN>::template ss<0, 0>(acc[mh], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | dyi | k) != 0);
+                mma_step<BN, TIn>(acc[mh], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | dyi | k) != 0);
               }
           }
         } else {
           const uint64_t db = make_smem_desc(sb, 16, 1024, SWZ_128B);
 #pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k)
+          for (int k = 0; k < kBlockK / 16; ++k)   // four 32-byte K steps: k16 bf16 or k32 e4m3
 #pragma unroll
             for (int mh = 0; mh < MH; ++mh) {   // PP: rows 64 mh.. of the A tile, 64 x 128 B further on
               const uint64_t da = make_smem_desc(sa + (uint32_t)(mh * 64 * 128), 16, 1024, SWZ_128B);
-              Wgmma<BN>::template ss<0, 0>(acc[mh], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) != 0);
+              mma_step<BN, TIn>(acc[mh], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) != 0);
             }
         }
         wgmma_commit();
@@ -501,12 +524,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
         long long m[2];
         bool row_ok[2];
         const float* b2[2];
+        float as[2] = {1.f, 1.f};   // e4m3: activation scale of the thread's two rows
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int r = rbase + 8 * h;
           m[h] = (long long)tile_m * p.rows_valid + r;
           row_ok[h] = r < p.rows_valid && m[h] < p.M;
           b2[h] = p.bias2 ? p.bias2 + (row_ok[h] ? (m[h] / p.bias2_div) : 0) * (long long)p.N : nullptr;
+          if constexpr (F8) as[h] = row_ok[h] ? __ldg(p.a_scale + m[h]) : 0.f;
           if constexpr (LNF) {
             if (p.ares) {
             } else if (p.ln_parts) {
@@ -540,10 +565,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
               sv = *reinterpret_cast<const float2*>(p.ln_colsum + nv);
               sg = *reinterpret_cast<const float2*>(p.ln_colsum + ng);
             }
+            float2 wv = make_float2(1.f, 1.f), wg2 = make_float2(1.f, 1.f);
+            if constexpr (F8) {
+              wv = __ldg(reinterpret_cast<const float2*>(p.w_scale + nv));
+              wg2 = __ldg(reinterpret_cast<const float2*>(p.w_scale + ng));
+            }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               float v0 = ac[4 * g + 2 * h], v1 = ac[4 * g + 2 * h + 1];
               float g0 = ac[4 * (g + G2) + 2 * h], g1 = ac[4 * (g + G2) + 2 * h + 1];
+              if constexpr (F8) {
+                v0 *= as[h] * wv.x;
+                v1 *= as[h] * wv.y;
+                g0 *= as[h] * wg2.x;
+                g1 *= as[h] * wg2.y;
+              }
               if constexpr (LNF) {
                 v0 = ln_rstd[h] * (v0 - ln_mean[h] * sv.x);
                 v1 = ln_rstd[h] * (v1 - ln_mean[h] * sv.y);
@@ -563,9 +599,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
             const float2 bv = p.bias ? *reinterpret_cast<const float2*>(p.bias + n) : make_float2(0.f, 0.f);
             float2 cs = make_float2(0.f, 0.f);
             if constexpr (LNF) cs = *reinterpret_cast<const float2*>(p.ln_colsum + n);
+            float2 ws = make_float2(1.f, 1.f);
+            if constexpr (F8) ws = __ldg(reinterpret_cast<const float2*>(p.w_scale + n));
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               float f0 = ac[4 * g + 2 * h], f1 = ac[4 * g + 2 * h + 1];
+              if constexpr (F8) {
+                f0 *= as[h] * ws.x;
+                f1 *= as[h] * ws.y;
+              }
               if constexpr (LNF) {
                 f0 = ln_rstd[h] * (f0 - ln_mean[h] * cs.x);
                 f1 = ln_rstd[h] * (f1 - ln_mean[h] * cs.y);
@@ -706,42 +748,70 @@ static int pick_block_n(long long tiles_m, int N, int gran, int total_kb, int fi
   return best;
 }
 
-template <int BN, bool LNF, bool PP>
+template <int BN, bool LNF, bool PP, typename TIn>
 static cudaError_t launch_bn(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mB, const CUtensorMap& mR,
                              const CUtensorMap& mC, const GemmArgs& a, int grid, size_t smem, cudaStream_t st) {
   static bool configured = false;
   if (!configured) {
-    const cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, LNF, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap);
+    const cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, LNF, PP, TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               kSmemCap);
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  return launch_k((gemm_wgmma_kernel<BN, LNF, PP>), dim3(grid), dim3(kThreads), smem, st, mA, mA2, mB, mR, mC, a);
+  return launch_k((gemm_wgmma_kernel<BN, LNF, PP, TIn>), dim3(grid), dim3(kThreads), smem, st, mA, mA2, mB, mR, mC, a);
 }
 
 template <bool LNF>
 static cudaError_t launch_lnf(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mB, const CUtensorMap& mR,
                               const CUtensorMap& mC, const GemmArgs& a, int grid, size_t smem, cudaStream_t st) {
+  using T = __nv_bfloat16;
   if constexpr (!LNF) {
     if (a.pp) {
       switch (a.block_n) {
-        case 32: return launch_bn<32, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-        case 64: return launch_bn<64, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-        case 96: return launch_bn<96, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-        case 128: return launch_bn<128, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-        case 160: return launch_bn<160, false, true>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        case 32: return launch_bn<32, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        case 64: return launch_bn<64, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        case 96: return launch_bn<96, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        case 128: return launch_bn<128, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+        case 160: return launch_bn<160, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
         default: return cudaErrorInvalidValue;
       }
     }
   }
   switch (a.block_n) {
-    case 16: return launch_bn<16, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 32: return launch_bn<32, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 64: return launch_bn<64, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 96: return launch_bn<96, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 128: return launch_bn<128, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 160: return launch_bn<160, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 192: return launch_bn<192, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
-    case 256: return launch_bn<256, LNF, false>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 16: return launch_bn<16, LNF, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 32: return launch_bn<32, LNF, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 64: return launch_bn<64, LNF, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 96: return launch_bn<96, LNF, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 128: return launch_bn<128, LNF, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 160: return launch_bn<160, LNF, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 192: return launch_bn<192, LNF, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 256: return launch_bn<256, LNF, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+// e4m3 operands (vx_gemm_fp8): the plain producer at the widths of bf16 output tiles (BN 16 is the fp32-output width)
+static cudaError_t launch_f8(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mB, const CUtensorMap& mR,
+                             const CUtensorMap& mC, const GemmArgs& a, int grid, size_t smem, cudaStream_t st) {
+  using T = __nv_fp8_e4m3;
+  if (a.pp) {
+    switch (a.block_n) {
+      case 32: return launch_bn<32, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+      case 64: return launch_bn<64, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+      case 96: return launch_bn<96, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+      case 128: return launch_bn<128, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+      case 160: return launch_bn<160, false, true, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+      default: return cudaErrorInvalidValue;
+    }
+  }
+  switch (a.block_n) {
+    case 32: return launch_bn<32, false, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 64: return launch_bn<64, false, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 96: return launch_bn<96, false, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 128: return launch_bn<128, false, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 160: return launch_bn<160, false, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 192: return launch_bn<192, false, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
+    case 256: return launch_bn<256, false, false, T>(mA, mA2, mB, mR, mC, a, grid, smem, st);
     default: return cudaErrorInvalidValue;
   }
 }
@@ -783,14 +853,17 @@ static int launch(const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorM
   VX_REQUIRE(smem <= (size_t)kSmemCap, "vx_gemm: %zu bytes of shared memory needed (bn=%d, K blocks=%d)", smem, a.block_n,
              a.kblocks1);
   if (gemm_env().verbose)
-    fprintf(stderr, "[vx_gemm] M=%d N=%d kb=%d taps=%d bn=%d pp=%d rr=%d stages=%d nbuf=%d tiles=%dx%d\n", a.M, a.N,
-            total_kb, a.taps, a.block_n, a.pp, a.rr, stages, nbuf, a.tiles_m, a.tiles_n);
+    fprintf(stderr, "[vx_gemm] M=%d N=%d kb=%d taps=%d bn=%d pp=%d rr=%d stages=%d nbuf=%d tiles=%dx%d%s\n", a.M, a.N,
+            total_kb, a.taps, a.block_n, a.pp, a.rr, stages, nbuf, a.tiles_m, a.tiles_n, a.a_scale ? " e4m3" : "");
   const int npar = a.ups ? 4 : 1;
   const bool lnf = a.ln_stats != nullptr || a.ln_parts != nullptr || a.ares;
   VX_REQUIRE(!a.pp || (!lnf && !a.rs_out && pp_bn_supported(a.block_n)), "vx_gemm: no ping-pong kernel for bn=%d", a.block_n);
   const long long tiles = a.ares ? a.tiles_m : (long long)a.tiles_m * a.tiles_n * npar;
   const int grid = tiles < device_sms() ? (int)tiles : device_sms();
+  VX_REQUIRE(!a.a_scale || (!lnf && !a.rs_out && a.taps == 1 && !a.kblocks2 && !a.out_f32 && a.block_n >= 32),
+             "vx_gemm_fp8: plain producer, linear / GEGLU bf16 epilogue, block_n >= 32 only");
   if (lnf) VX_CHECK_CUDA((launch_lnf<true>(mA, mA2, mB, mR, mC, a, grid, smem, st)));
+  else if (a.a_scale) VX_CHECK_CUDA((launch_f8(mA, mA2, mB, mR, mC, a, grid, smem, st)));
   else VX_CHECK_CUDA((launch_lnf<false>(mA, mA2, mB, mR, mC, a, grid, smem, st)));
   VX_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -836,20 +909,26 @@ static int gemm_entry(const void* A, long long lda, int K1, const void* A2, long
                       long long ldw, int M, int N, const float* bias, const float* bias2, int bias2_div, float scale,
                       const void* residual, long long ldr, void* out, long long ldc, int out_f32, int block_n,
                       const float* ln_stats, const float* ln_colsum, void* stream, float ln_eps = 0.f,
-                      const RowStatsIO* rs = nullptr) {
+                      const RowStatsIO* rs = nullptr, const float* a_scale = nullptr, const float* w_scale = nullptr) {
   const int geglu = out_f32 == 2 ? 1 : 0;  // out_f32: 0 bf16, 1 fp32, 2 bf16 + GEGLU epilogue
   const bool ares = ln_colsum && !ln_stats && !(rs && rs->parts);   // LayerNorm GEMM with in-kernel statistics (A tile resident)
+  // operand element size: 2 (bf16), or 1 (e4m3 with per-row / per-column scales): K blocks of kKE elements = 128 bytes
+  const bool f8 = a_scale != nullptr;
+  const int esz = f8 ? 1 : 2, kKE = kBlockK * 2 / esz;
+  const CUtensorMapDataType tdt = f8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   if (geglu) out_f32 = 0;
   VX_REQUIRE(M > 0 && N > 0 && K1 > 0, "vx_gemm_bf16: bad shape M=%d N=%d K1=%d", M, N, K1);
   const int gran = geglu ? 64 : (out_f32 ? 16 : 32);
   VX_REQUIRE(N % gran == 0, "vx_gemm_bf16: N=%d must be a multiple of %d", N, gran);
-  VX_REQUIRE(K1 % 8 == 0 && K2 % 8 == 0 && lda % 8 == 0 && ldw % 8 == 0 && ldc % 8 == 0,
-             "vx_gemm_bf16: K/ld must be multiples of 8 elements (16-byte TMA strides)");
+  VX_REQUIRE(K1 % (16 / esz) == 0 && K2 % 8 == 0 && lda % (16 / esz) == 0 && ldw % (16 / esz) == 0 && ldc % 8 == 0,
+             "vx_gemm: K/ld must be multiples of 16 bytes (TMA strides), ldc of 8 elements");
+  VX_REQUIRE(!f8 || (w_scale && K2 == 0 && !out_f32 && !ln_colsum && !ln_stats && !rs),
+             "vx_gemm_fp8: w_scale missing, or an operand mode the e4m3 GEMM does not have");
   VX_REQUIRE(K2 == 0 || (K1 % kBlockK == 0 && lda2 % 8 == 0), "vx_gemm_bf16: split-K needs K1 %% 64 == 0");
   VX_REQUIRE(!residual || (ldr % 8 == 0 && !out_f32 && !geglu), "vx_gemm_bf16: residual needs bf16 linear epilogue, ldr %%8");
   VX_REQUIRE(!geglu || (!bias2 && scale == 1.0f), "vx_gemm_bf16: GEGLU epilogue takes only the packed bias");
   const int tiles_m = (M + kBlockM - 1) / kBlockM;
-  const int total_kb = (K1 + kBlockK - 1) / kBlockK + (K2 + kBlockK - 1) / kBlockK;
+  const int total_kb = (K1 + kKE - 1) / kKE + (K2 + kBlockK - 1) / kBlockK;
   if (block_n <= 0) block_n = gemm_env().bn;
   if (ares) {
     VX_REQUIRE(K2 == 0 && K1 % kBlockK == 0 && K1 <= 8 * kBlockK && !out_f32,
@@ -887,9 +966,9 @@ static int gemm_entry(const void* A, long long lda, int K1, const void* A2, long
   CUtensorMap mA, mA2, mB, mR, mC;
   {
     uint64_t dims[2] = {(uint64_t)K1, (uint64_t)M};
-    uint64_t str[1] = {(uint64_t)lda * 2};
-    uint32_t box[2] = {kBlockK, kBlockM};
-    if (make_tmap_bf16(&mA, A, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+    uint64_t str[1] = {(uint64_t)lda * esz};
+    uint32_t box[2] = {(uint32_t)kKE, kBlockM};
+    if (make_tmap_bf16(&mA, A, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, tdt)) return 1;
   }
   if (K2 > 0) {
     uint64_t dims[2] = {(uint64_t)K2, (uint64_t)M};
@@ -901,9 +980,9 @@ static int gemm_entry(const void* A, long long lda, int K1, const void* A2, long
   }
   {
     uint64_t dims[2] = {(uint64_t)(K1 + K2), (uint64_t)N};
-    uint64_t str[1] = {(uint64_t)ldw * 2};
-    uint32_t box[2] = {kBlockK, (uint32_t)block_n};
-    if (make_tmap_bf16(&mB, Wt, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+    uint64_t str[1] = {(uint64_t)ldw * esz};
+    uint32_t box[2] = {(uint32_t)kKE, (uint32_t)block_n};
+    if (make_tmap_bf16(&mB, Wt, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, tdt)) return 1;
   }
   if (!out_f32) {
     if (make_out_maps(&mR, &mC, residual, ldr, out, ldc, M, geglu ? N / 2 : N, kBlockM)) return 1;
@@ -913,9 +992,11 @@ static int gemm_entry(const void* A, long long lda, int K1, const void* A2, long
   }
   GemmArgs a{};
   a.M = M; a.N = N;
-  a.kblocks1 = (K1 + kBlockK - 1) / kBlockK;
+  a.kblocks1 = (K1 + kKE - 1) / kKE;
   a.kblocks2 = (K2 + kBlockK - 1) / kBlockK;
   a.taps = 1;
+  a.a_scale = a_scale;
+  a.w_scale = w_scale;
   a.block_n = block_n;
   a.pp = pp;
   a.rows_valid = kBlockM;
@@ -954,6 +1035,18 @@ extern "C" int vx_gemm_bf16(const void* A, long long lda, int K1, const void* A2
                             long long ldc, int out_f32, int block_n, void* stream) {
   return gemm_entry(A, lda, K1, A2, lda2, K2, Wt, ldw, M, N, bias, bias2, bias2_div, scale, residual, ldr, out, ldc,
                     out_f32, block_n, nullptr, nullptr, stream);
+}
+
+// e4m3 operands with per-row / per-output-channel scales: out = epilogue(sum_k A[m,k] W[n,k] * a_scale[m] * w_scale[n]),
+// the epilogue (bias, bias2, scale, residual; or GEGLU with W, w_scale and bias packed as for vx_gemm_bf16) as in
+// vx_gemm_bf16.  A [M, K] and W [N, K] hold float8_e4m3fn codes, K-major; K, lda, ldw multiples of 16.
+extern "C" int vx_gemm_fp8(const void* A, long long lda, const float* a_scale, int K, const void* Wt, long long ldw,
+                           const float* w_scale, int M, int N, const float* bias, const float* bias2, int bias2_div,
+                           float scale, const void* residual, long long ldr, void* out, long long ldc, int geglu,
+                           int block_n, void* stream) {
+  VX_REQUIRE(a_scale && w_scale, "vx_gemm_fp8: a_scale / w_scale missing (M=%d N=%d)", M, N);
+  return gemm_entry(A, lda, K, nullptr, 0, 0, Wt, ldw, M, N, bias, bias2, bias2_div, scale, residual, ldr, out, ldc,
+                    geglu ? 2 : 0, block_n, nullptr, nullptr, stream, 0.f, nullptr, a_scale, w_scale);
 }
 
 // LayerNorm folded into the GEMM: A holds the UN-normalised rows, Wt = W * gamma (per input channel),

@@ -42,9 +42,11 @@ int device_sms();  // multiprocessors of the current device (vx_runtime.cu)
 // bf16 tensor map of rank `rank`: dims[i] elements, strides_bytes[i-1] for i>=1, box[i] elements.
 // estrides (optional): traversal stride per dimension (1..8): the box then covers box[i] tensor elements of which every
 // estrides[i]-th is loaded, i.e. box[i] / estrides[i] elements land in shared memory (the stride-2 convolutions).
+// dtype: CU_TENSOR_MAP_DATA_TYPE_UINT8 for the e4m3 operands of vx_gemm_fp8 (TMA only moves bytes).
 inline int make_tmap_bf16(CUtensorMap* m, const void* base, int rank, const uint64_t* dims,
                           const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swz,
-                          const uint32_t* estrides = nullptr) {
+                          const uint32_t* estrides = nullptr,
+                          CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) return fail("cuTensorMapEncodeTiled entry point unavailable");
   cuuint64_t gd[5];
@@ -57,7 +59,7 @@ inline int make_tmap_bf16(CUtensorMap* m, const void* base, int rank, const uint
     es[i] = estrides ? estrides[i] : 1;
     if (i) gs[i - 1] = strides_bytes[i - 1];
   }
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
+  CUresult r = enc(m, dtype, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)

@@ -6,7 +6,8 @@
 //     Reference: InflatedGroupNorm modules/resnet.py:20-28, ResnetBlock3D.forward :220-221,235-241,
 //     Transformer3DModel.forward modules/transformer_3d.py:124, TemporalTransformer3DModel modules/motion_module.py:156.
 //   * LayerNorm over C (eps 1e-5) with the optional sinusoidal positional-encoding add of the temporal
-//     attention (reference modules/motion_module.py:244,262-277,365-366; attention.py:329-333).
+//     attention (reference modules/motion_module.py:244,262-277,365-366; attention.py:329-333).  The e4m3 form
+//     (vx_layernorm_fp8) writes float8_e4m3fn codes of the fp32 result and one scale per row, amax(|row|) / 448.
 //   * GEGLU gate: out = h * gelu_erf(gate) (diffusers FeedForward/GEGLU, SURVEY.md Appendix B.3).
 // All loads/stores are 16-byte vectors, threads walk the contiguous channel dimension.
 #include "vx_host.h"
@@ -28,6 +29,20 @@ __device__ __forceinline__ void store8(__nv_bfloat16* p, const float (&f)[8]) {
   *reinterpret_cast<uint4*>(p) =
       make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
 }
+// two e4m3 codes (round to nearest even, saturated to +-448): a in the low byte, b in the high byte
+__device__ __forceinline__ uint32_t pack_e4m3x2(float a, float b) {
+  uint16_t d;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(d) : "f"(b), "f"(a));
+  return d;
+}
+// f[j] * inv as eight e4m3 codes (8 bytes)
+__device__ __forceinline__ void store8_e4m3(uint8_t* p, const float (&f)[8], float inv) {
+  const uint32_t lo = pack_e4m3x2(f[0] * inv, f[1] * inv) | pack_e4m3x2(f[2] * inv, f[3] * inv) << 16;
+  const uint32_t hi = pack_e4m3x2(f[4] * inv, f[5] * inv) | pack_e4m3x2(f[6] * inv, f[7] * inv) << 16;
+  *reinterpret_cast<uint2*>(p) = make_uint2(lo, hi);
+}
+// e4m3 row scale from the row's amax: codes are value / scale, the largest one 448 (the e4m3 maximum); an all-zero row gets 1
+__device__ __forceinline__ float e4m3_row_scale(float amax) { return amax > 0.f ? amax / 448.f : 1.f; }
 
 // ------------------------------------------------------------------ GroupNorm statistics
 // grid (S, NB); block = V*R threads (V = C/8 vectors per pixel, R pixel rows in flight).
@@ -429,11 +444,13 @@ __global__ void gn_cluster_kernel(const GnClusterArgs p) {
 
 // ------------------------------------------------------------------ LayerNorm (+PE)
 // One warp per row; the row lives in registers (C <= 2048), exact two-pass mean/variance like torch.
-template <int MAXV>
+// TOut = uint8_t: e4m3 codes of the fp32 result and row_scale[row] (vx_layernorm_fp8).
+template <int MAXV, typename TOut>
 __global__ void layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int rows, int C,
                                  const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
                                  const float* __restrict__ pe, int pe_rows_per_frame, int pe_frames,
-                                 __nv_bfloat16* __restrict__ out, long long ldo) {
+                                 TOut* __restrict__ out, long long ldo, float* __restrict__ row_scale) {
+  constexpr bool F8 = sizeof(TOut) == 1;
   pdl_enter();
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -470,22 +487,45 @@ __global__ void layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long 
   const float rstd = rsqrtf(q / C + eps);
   const float* perow = nullptr;
   if (pe) perow = pe + (long long)((warp / pe_rows_per_frame) % pe_frames) * C;
+  auto norm8 = [&](int i, int v, float (&y)[8]) {
+    const float4 g0 = *reinterpret_cast<const float4*>(gamma + v * 8), g1 = *reinterpret_cast<const float4*>(gamma + v * 8 + 4);
+    const float4 b0 = *reinterpret_cast<const float4*>(beta + v * 8), b1 = *reinterpret_cast<const float4*>(beta + v * 8 + 4);
+    const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) y[j] = (f[i][j] - mean) * rstd * gg[j] + bb[j];
+    if (perow) {
+      const float4 p0 = *reinterpret_cast<const float4*>(perow + v * 8), p1 = *reinterpret_cast<const float4*>(perow + v * 8 + 4);
+      y[0] += p0.x; y[1] += p0.y; y[2] += p0.z; y[3] += p0.w; y[4] += p1.x; y[5] += p1.y; y[6] += p1.z; y[7] += p1.w;
+    }
+  };
+  float inv = 1.f;
+  if constexpr (F8) {   // amax pass over the normalised row; the write pass recomputes the same fp32 values
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      const int v = lane + i * 32;
+      if (v < V) {
+        float y[8];
+        norm8(i, v, y);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(y[j]));
+      }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const float sc = e4m3_row_scale(amax);
+    inv = 1.0f / sc;
+    if (lane == 0) row_scale[warp] = sc;
+  }
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
     const int v = lane + i * 32;
     if (v < V) {
       float y[8];
-      const float4 g0 = *reinterpret_cast<const float4*>(gamma + v * 8), g1 = *reinterpret_cast<const float4*>(gamma + v * 8 + 4);
-      const float4 b0 = *reinterpret_cast<const float4*>(beta + v * 8), b1 = *reinterpret_cast<const float4*>(beta + v * 8 + 4);
-      const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-      const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-      for (int j = 0; j < 8; ++j) y[j] = (f[i][j] - mean) * rstd * gg[j] + bb[j];
-      if (perow) {
-        const float4 p0 = *reinterpret_cast<const float4*>(perow + v * 8), p1 = *reinterpret_cast<const float4*>(perow + v * 8 + 4);
-        y[0] += p0.x; y[1] += p0.y; y[2] += p0.z; y[3] += p0.w; y[4] += p1.x; y[5] += p1.y; y[6] += p1.z; y[7] += p1.w;
-      }
-      store8(out + (long long)warp * ldo + v * 8, y);
+      norm8(i, v, y);
+      if constexpr (F8) store8_e4m3(out + (long long)warp * ldo + v * 8, y, inv);
+      else store8(out + (long long)warp * ldo + v * 8, y);
     }
   }
 }
@@ -551,12 +591,15 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
 // five 16-byte vectors per lane (no idle lanes, 128-byte coalesced segments), 32 / LPR rows per warp pass.  gamma and
 // beta live in registers for the whole grid-stride loop: the per-row version above spends four parameter loads per
 // data load on them.
-template <int LPR, int MINB>
+// TOut = uint8_t: e4m3 codes of the fp32 result and row_scale[row] (vx_layernorm_fp8).
+template <int LPR, int MINB, typename TOut>
 __global__ void __launch_bounds__(256, MINB) layernorm5_kernel(const __nv_bfloat16* __restrict__ x, long long ldx,
                                                             long long rows, const float* __restrict__ gamma,
                                                             const float* __restrict__ beta, float eps,
                                                             const float* __restrict__ pe, int pe_rows_per_frame,
-                                                            int pe_frames, __nv_bfloat16* __restrict__ out, long long ldo) {
+                                                            int pe_frames, TOut* __restrict__ out, long long ldo,
+                                                            float* __restrict__ row_scale) {
+  constexpr bool F8 = sizeof(TOut) == 1;
   pdl_enter();
   constexpr int RPW = 32 / LPR;
   constexpr int C = LPR * 40;
@@ -618,11 +661,9 @@ __global__ void __launch_bounds__(256, MINB) layernorm5_kernel(const __nv_bfloat
       for (int o = LPR / 2; o; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
       const float rstd = rsqrtf(q * (1.0f / C) + eps);
       const float* perow = pe ? pe + (long long)((row[r] / pe_rows_per_frame) % pe_frames) * C + l * 8 : nullptr;
-      __nv_bfloat16* op = out + (ok[r] ? row[r] : 0) * ldo + l * 8;
-#pragma unroll
-      for (int i = 0; i < 5; ++i) {
+      TOut* op = out + (ok[r] ? row[r] : 0) * ldo + l * 8;
+      auto norm8 = [&](int i, float (&y)[8]) {
         const uint32_t w4[4] = {u[r][i].x, u[r][i].y, u[r][i].z, u[r][i].w};
-        float y[8];
         int c = (l + i * LPR) * 8;
         asm volatile("" : "+r"(c));     // opaque to the optimiser: or it hoists all 80 parameter loads out of the row loop again
         const float4 g0 = *reinterpret_cast<const float4*>(sg + c), g1 = *reinterpret_cast<const float4*>(sg + c + 4);
@@ -640,7 +681,32 @@ __global__ void __launch_bounds__(256, MINB) layernorm5_kernel(const __nv_bfloat
           const float4 p1 = *reinterpret_cast<const float4*>(perow + i * LPR * 8 + 4);
           y[0] += p0.x; y[1] += p0.y; y[2] += p0.z; y[3] += p0.w; y[4] += p1.x; y[5] += p1.y; y[6] += p1.z; y[7] += p1.w;
         }
-        if (ok[r]) store8(op + i * LPR * 8, y);
+      };
+      if constexpr (F8) {   // the lane's 40 normalised values stay in registers until the row's amax is known
+        float y[5][8];
+        float amax = 0.f;
+#pragma unroll
+        for (int i = 0; i < 5; ++i) {
+          norm8(i, y[i]);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(y[i][j]));
+        }
+#pragma unroll
+        for (int o = LPR / 2; o; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+        const float sc = e4m3_row_scale(amax);
+        const float inv = 1.0f / sc;
+        if (ok[r]) {
+#pragma unroll
+          for (int i = 0; i < 5; ++i) store8_e4m3(op + i * LPR * 8, y[i], inv);
+          if (l == 0) row_scale[row[r]] = sc;
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < 5; ++i) {
+          float y[8];
+          norm8(i, y);
+          if (ok[r]) store8(op + i * LPR * 8, y);
+        }
       }
     }
   }
@@ -908,16 +974,20 @@ extern "C" int vx_groupnorm_cluster(const void* x1, long long ld1, int C1, const
   return 0;
 }
 
-// pe: optional float [pe_frames, C]; row r uses pe[(r / rows_per_frame) % pe_frames]
-extern "C" int vx_layernorm(const void* x, long long ldx, long long rows, int C, const float* gamma,
-                            const float* beta, float eps, const float* pe, int rows_per_frame, int pe_frames,
-                            void* out, long long ldo, void* stream) {
-  VX_REQUIRE(C % 8 == 0 && C <= 2048, "vx_layernorm: C=%d unsupported", C);
+// pe: optional float [pe_frames, C]; row r uses pe[(r / rows_per_frame) % pe_frames].  TOut = uint8_t: e4m3 codes + row_scale.
+template <typename TOut>
+static int layernorm_entry(const void* x, long long ldx, long long rows, int C, const float* gamma, const float* beta,
+                           float eps, const float* pe, int rows_per_frame, int pe_frames, void* out, long long ldo,
+                           float* row_scale, void* stream) {
+  constexpr bool F8 = sizeof(TOut) == 1;
+  const char* name = F8 ? "vx_layernorm_fp8" : "vx_layernorm";
+  VX_REQUIRE(C % 8 == 0 && C <= 2048, "%s: C=%d unsupported", name, C);
+  VX_REQUIRE(!F8 || (row_scale && ldo % 8 == 0), "vx_layernorm_fp8: row_scale missing or ldo %% 8 != 0");
   const int threads = 256;
   const long long blocks = (rows * 32 + threads - 1) / threads;
   const int V = C / 8;
   auto st = (cudaStream_t)stream;
-  if (pe && (rows_per_frame <= 0 || pe_frames <= 0)) return fail("vx_layernorm: bad pe args");
+  if (pe && (rows_per_frame <= 0 || pe_frames <= 0)) return fail("%s: bad pe args", name);
   // The positional-encoding variant (temporal attention norms) takes the same kernel since its parameters moved to shared
   // memory: 63.5 -> ~41 us at the 320-wide level (the one-warp-per-row kernel used to be as fast).  VX_LN_PE5=0: old choice.
   static const bool ln_v1 = getenv("VX_LN_V1") != nullptr;   // A/B switch, read once
@@ -926,17 +996,20 @@ extern "C" int vx_layernorm(const void* x, long long ldx, long long rows, int C,
     const int lpr = C / 40;
     const long long groups = (rows + 32 / lpr - 1) / (32 / lpr);
     long long nb = ((groups + 1) / 2 + 7) / 8;
-    static const int minb = getenv("VX_LN_BLOCKS") ? atoi(getenv("VX_LN_BLOCKS")) : 3;   // read once (A/B switch)
+    static const int minb_env = getenv("VX_LN_BLOCKS") ? atoi(getenv("VX_LN_BLOCKS")) : 3;   // read once (A/B switch)
+    // e4m3: the lane's 40 normalised values wait in registers for the row amax -- two blocks per SM (three spill)
+    const int minb = F8 ? 2 : minb_env;
     if (nb > device_sms() * minb * 2) nb = device_sms() * minb * 2;   // `minb` 256-thread blocks are resident per SM; two waves balance the tail
     if (nb < 1) nb = 1;
 #define LN5_LAUNCH(LPR)                                                                                               \
   do {                                                                                                               \
-    if (minb == 2)                                                                                                   \
-      launch_k((layernorm5_kernel<LPR, 2>), dim3((unsigned)nb), dim3(256), 0, st, (const __nv_bfloat16*)x, ldx, rows, gamma, beta, eps, pe, \
-                                                              rows_per_frame, pe_frames, (__nv_bfloat16*)out, ldo);  \
-    else                                                                                                             \
-      launch_k((layernorm5_kernel<LPR, 3>), dim3((unsigned)nb), dim3(256), 0, st, (const __nv_bfloat16*)x, ldx, rows, gamma, beta, eps, pe, \
-                                                              rows_per_frame, pe_frames, (__nv_bfloat16*)out, ldo);  \
+    if (minb == 2) {                                                                                                 \
+      launch_k((layernorm5_kernel<LPR, 2, TOut>), dim3((unsigned)nb), dim3(256), 0, st, (const __nv_bfloat16*)x, ldx, rows, gamma, beta, \
+               eps, pe, rows_per_frame, pe_frames, (TOut*)out, ldo, row_scale);                                      \
+    } else if constexpr (!F8) {                                                                                      \
+      launch_k((layernorm5_kernel<LPR, 3, TOut>), dim3((unsigned)nb), dim3(256), 0, st, (const __nv_bfloat16*)x, ldx, rows, gamma, beta, \
+               eps, pe, rows_per_frame, pe_frames, (TOut*)out, ldo, row_scale);                                      \
+    }                                                                                                                \
   } while (0)
     if (lpr == 8) LN5_LAUNCH(8);
     else if (lpr == 16) LN5_LAUNCH(16);
@@ -946,9 +1019,8 @@ extern "C" int vx_layernorm(const void* x, long long ldx, long long rows, int C,
     return 0;
   }
 #define LN_LAUNCH(MV)                                                                                            \
-  launch_k(layernorm_kernel<MV>, dim3((unsigned)blocks), dim3(threads), 0, st, (const __nv_bfloat16*)x, ldx, (int)rows, C, gamma, \
-                                                             beta, eps, pe, rows_per_frame, pe_frames,          \
-                                                             (__nv_bfloat16*)out, ldo)
+  launch_k(layernorm_kernel<MV, TOut>, dim3((unsigned)blocks), dim3(threads), 0, st, (const __nv_bfloat16*)x, ldx, (int)rows, C, \
+           gamma, beta, eps, pe, rows_per_frame, pe_frames, (TOut*)out, ldo, row_scale)
   if (V <= 32) LN_LAUNCH(1);
   else if (V <= 64) LN_LAUNCH(2);
   else if (V <= 96) LN_LAUNCH(3);
@@ -957,6 +1029,22 @@ extern "C" int vx_layernorm(const void* x, long long ldx, long long rows, int C,
 #undef LN_LAUNCH
   VX_CHECK_CUDA(cudaGetLastError());
   return 0;
+}
+
+extern "C" int vx_layernorm(const void* x, long long ldx, long long rows, int C, const float* gamma,
+                            const float* beta, float eps, const float* pe, int rows_per_frame, int pe_frames,
+                            void* out, long long ldo, void* stream) {
+  return layernorm_entry<__nv_bfloat16>(x, ldx, rows, C, gamma, beta, eps, pe, rows_per_frame, pe_frames, out, ldo, nullptr,
+                                        stream);
+}
+
+// LayerNorm (+ pe) -> float8_e4m3fn codes out[row, c] = sat_rn(y / row_scale[row]) of the fp32 result y (no bf16 rounding
+// on the way), row_scale[row] = amax_c |y| / 448 (1 for an all-zero row): the A operand of vx_gemm_fp8.
+extern "C" int vx_layernorm_fp8(const void* x, long long ldx, long long rows, int C, const float* gamma,
+                                const float* beta, float eps, const float* pe, int rows_per_frame, int pe_frames,
+                                void* out, long long ldo, float* row_scale, void* stream) {
+  return layernorm_entry<uint8_t>(x, ldx, rows, C, gamma, beta, eps, pe, rows_per_frame, pe_frames, out, ldo, row_scale,
+                                  stream);
 }
 
 // x: [rows, 2*inner] = (h | gate) -> out [rows, inner]

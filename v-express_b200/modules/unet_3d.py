@@ -256,6 +256,7 @@ class UNet3DConditionModel(nn.Module):
         _build_tree(self, _unet_keys(tuple(block_out_channels), cross_attention_dim, layers_per_block, in_channels,
                                      out_channels, self.pe_len))
         self._engine: Optional[UNetEngine] = None
+        self._fp8_linear = False
         self.reference_attention_weight = 1.0
         self.audio_attention_weight = 1.0
 
@@ -308,6 +309,26 @@ class UNet3DConditionModel(nn.Module):
             self._engine = UNetEngine(self)
         return self._engine
 
+    # ---- opt-in FP8 (e4m3) for the Linears that read a LayerNorm output (DESIGN section 3, "FP8 mode")
+    def enable_fp8_linear(self):
+        """Run every Linear fed by a LayerNorm -- the fused q|k|v, attn1_5.to_q, attn2.to_q and the GEGLU projection of the
+        spatial transformer blocks, the fused q|k|v and the GEGLU projection of the motion modules -- on e4m3 operands: the
+        LayerNorm writes e4m3 codes with one scale per row, the weights are quantised per output channel.  Lossy (about 7.5 %
+        relative L2 error of the noise prediction on the reduced-width test UNet, against 0.5 % for bf16): off by default.
+        The e4m3 weights are packed next to the bf16 ones and rebuilt on every load_state_dict / .to."""
+        _check_fp8_env()
+        self._fp8_linear = True
+        if self._engine is not None:
+            self._engine.set_fp8(True)
+        return self
+
+    def disable_fp8_linear(self):
+        """Back to the bf16 path (bit-identical to a model that never enabled FP8)."""
+        self._fp8_linear = False
+        if self._engine is not None:
+            self._engine.set_fp8(False)
+        return self
+
     @torch.no_grad()
     def forward(self, sample, timestep, encoder_hidden_states, class_labels=None, kps_features=None,
                 attention_mask=None, down_block_additional_residuals=None, mid_block_additional_residual=None,
@@ -335,11 +356,24 @@ class UNet3DConditionModel(nn.Module):
         return UNet3DConditionOutput(sample=out)
 
 
+def _check_fp8_env():
+    for var in ("VX_LN_FOLD", "VX_LN_FUSE"):
+        if os.environ.get(var, "0") not in ("", "0"):
+            raise ValueError(f"enable_fp8_linear: {var} is set; that path normalises inside a bf16 GEMM, which has no "
+                             f"e4m3 form -- unset it to use FP8")
+
+
+# Linears that read a LayerNorm output (engine weight keys): the FP8 mode's coverage
+_FP8_KEYS = (".qkv", ".attn1_5.to_q.weight", ".attn2.to_q.weight", ".ff.net.0.proj.geglu_w")
+
+
 # ----------------------------------------------------------------------------------------------
 # the engine: packed weights + kernel schedule
 # ----------------------------------------------------------------------------------------------
 class UNetEngine:
     """Owns the packed (kernel-layout) weights of one model instance and runs the forward schedule."""
+
+    fp8 = False   # FP8 mode, off unless set_fp8(True) (the dry-run tests build engines without __init__)
 
     def __init__(self, model: UNet3DConditionModel):
         from .. import _ffi
@@ -361,6 +395,8 @@ class UNetEngine:
         self.W: Dict[str, torch.Tensor] = {}
         self._pack(sd)
         self._pack_ln_fold()
+        self.W8: Dict[str, tuple] = {}            # the e4m3 weights, packed on first use of the FP8 mode
+        self.set_fp8(model._fp8_linear)
         self._bank_cache: Dict[str, tuple] = {}
         self._bank_buf: Dict[str, torch.Tensor] = {}
         self._bank_flag: Dict[str, bool] = {}
@@ -460,6 +496,15 @@ class UNetEngine:
                     # (LayerNorm(x) + pe) W^T = LayerNorm(x) W^T + pe W^T: the positional encoding becomes a per-frame bias
                     self._pe_proj[a_] = (W[a_ + ".pos_encoder.pe"] @ W[a_ + ".qkv"].float().t()).contiguous()
 
+    def set_fp8(self, on: bool):
+        """FP8 mode on / off; the e4m3 weights (ops.quantize_fp8_weight of the packed bf16 ones) are made on first use."""
+        if on:
+            _check_fp8_env()
+            if not self.W8:
+                # per output channel, so the packed q|k|v and GEGLU (value | gate) orders carry over to codes and scales
+                self.W8 = {k: ops.quantize_fp8_weight(v) for k, v in self.W.items() if k.endswith(_FP8_KEYS)}
+        self.fp8 = bool(on)
+
     def _gemm_p(self, a, w, bias, **kw):
         """A Linear whose output feeds a LayerNorm: (out, hand-over) -- the hand-over is the (parts, nparts) of
         ops.gemm_rowsums under the statistics hand-over, else None."""
@@ -471,9 +516,16 @@ class UNetEngine:
     def _ln_gemm(self, h, norm_key, w_key, *, geglu=False, pe=None, rows_per_frame=0, b=1, rs=None):
         """LayerNorm(h) [+ pe] -> Linear.  Default: the LayerNorm kernel followed by the GEMM.  With the producer's row sums
         `rs` (VX_LN_FUSE=1): one GEMM with the normalising epilogue; VX_LN_FOLD=1: statistics kernel + GEMM with the
-        normalising epilogue."""
+        normalising epilogue.  FP8 mode: the LayerNorm writes e4m3 codes + row scales, the GEMM runs on e4m3 operands."""
         W = self.W
-        K = h.shape[1]
+        if self.fp8:
+            a8, a_scale = ops.layernorm_fp8(h, W[norm_key + ".weight"], W[norm_key + ".bias"], pe=pe,
+                                            rows_per_frame=rows_per_frame)
+            if geglu:
+                w8, w_scale = self.W8[w_key + ".geglu_w"]
+                return ops.gemm_fp8(a8, a_scale, w8, w_scale, W[w_key + ".geglu_b"], geglu=True)
+            w8, w_scale = self.W8[w_key]
+            return ops.gemm_fp8(a8, a_scale, w8, w_scale)
         if rs is None and not self.ln_fold:
             n = ops.layernorm(h, W[norm_key + ".weight"], W[norm_key + ".bias"], pe=pe, rows_per_frame=rows_per_frame)
             if geglu:
@@ -525,7 +577,7 @@ class UNetEngine:
 
     def graph_signature(self):
         """Changes whenever a CUDA graph captured from forward_frames would be stale."""
-        return (id(self), self.bank_epoch)
+        return (id(self), self.bank_epoch, self.fp8)
 
     # ---------------------------------------------------------------- blocks
     def _groupnorm(self, x, NB, HW, gamma, beta, eps, silu, x2=None, n=1):

@@ -105,6 +105,49 @@ def gemm(a, w, bias=None, *, a2=None, bias2=None, bias2_div=1, scale=1.0, residu
     return out
 
 
+# ---- FP8 (e4m3) operands with per-row / per-output-channel scales (opt-in: UNet3DConditionModel.enable_fp8_linear)
+E4M3 = torch.float8_e4m3fn
+E4M3_MAX = 448.0
+
+
+def quantize_fp8_weight(w):
+    """[N, K] weight -> (float8_e4m3fn codes [N, K], fp32 scale [N]): scale[n] = amax_k |w[n, k]| / 448 (1 for an all-zero
+    row), codes = clamp(w / scale, +-448) cast to e4m3 (round to nearest even; torch's cast does not saturate, hence the
+    clamp).  Per output channel, so a fused q|k|v weight carries the concatenated scales of q, k and v, and a weight packed
+    by pack_geglu gets codes and scales in its (value | gate) tile order."""
+    wf = w.float()
+    amax = wf.abs().amax(dim=1)
+    scale = torch.where(amax > 0, amax / E4M3_MAX, torch.ones_like(amax))
+    codes = (wf / scale[:, None]).clamp(-E4M3_MAX, E4M3_MAX).to(E4M3).contiguous()
+    return codes, scale.contiguous()
+
+
+def gemm_fp8(a, a_scale, w, w_scale, bias=None, *, bias2=None, bias2_div=1, scale=1.0, residual=None, out=None,
+             block_n=0, geglu=False):
+    """gemm() on e4m3 operands: out = epilogue(a_scale[m] * w_scale[n] * (a @ w.T)[m, n]) in bf16.  a [M, K] / w [N, K]
+    float8_e4m3fn (K a multiple of 16), a_scale [M] / w_scale [N] fp32; bias, bias2, scale, residual and geglu (w, w_scale
+    and bias packed by pack_geglu) as in gemm()."""
+    for t in (a, w):
+        assert t.is_cuda and t.dtype == E4M3 and t.stride(-1) == 1, (t.dtype, t.device, t.stride())
+    _chk_bf16(residual, out)
+    M, K = a.shape
+    N = w.shape[0]
+    assert w.shape[1] == K
+    for name, t, n in (("a_scale", a_scale, M), ("w_scale", w_scale, N)):
+        if t.dtype != torch.float32 or t.device != a.device or not t.is_contiguous() or t.shape != (n,) or t.data_ptr() % 8:
+            raise ValueError(f"{name} must be a contiguous fp32 [{n}] vector on {a.device}, got {t.dtype} {tuple(t.shape)}")
+    _chk_bias(bias, N, a.device, bias2, M, bias2_div)
+    if geglu and not block_n:
+        block_n = geglu_block_n(N)
+    if out is None:
+        out = torch.empty((M, N // 2 if geglu else N), device=a.device, dtype=BF16)
+    check(_ffi.lib().vx_gemm_fp8(
+        ptr(a), c_ll(a.stride(0)), ptr(a_scale), c_int(K), ptr(w), c_ll(w.stride(0)), ptr(w_scale), c_int(M), c_int(N),
+        ptr(bias), ptr(bias2), c_int(bias2_div), c_float(scale), ptr(residual), c_ll(0 if residual is None else residual.stride(0)),
+        ptr(out), c_ll(out.stride(0)), c_int(int(geglu)), c_int(block_n), stream_ptr()), "vx_gemm_fp8")
+    return out
+
+
 # ---- LayerNorm folded into the consumer GEMM (experiment; the engine uses it only under VX_LN_FOLD=1)
 def row_stats(x, eps=1e-5, out=None):
     """(mean, rstd) of every row of x [rows, C] bf16 -> fp32 [rows, 2]."""
@@ -476,6 +519,36 @@ def layernorm(x, gamma, beta, eps=1e-5, pe=None, rows_per_frame=0, out=None):
                                   c_float(eps), ptr(pe), c_int(rows_per_frame), c_int(0 if pe is None else pe.shape[0]),
                                   ptr(out), c_ll(out.stride(0)), stream_ptr()), "vx_layernorm")
     return out
+
+
+def layernorm_fp8(x, gamma, beta, eps=1e-5, pe=None, rows_per_frame=0, out=None, row_scale=None):
+    """layernorm() as the A operand of gemm_fp8: (float8_e4m3fn codes [rows, C], fp32 row_scale [rows]) with
+    codes * row_scale ~ LayerNorm(x) [+ pe] computed in fp32, row_scale = amax(|row|) / 448 (1 for an all-zero row)."""
+    _chk_bf16(x)
+    rows, C = x.shape
+    if out is None:
+        out = torch.empty((rows, C), device=x.device, dtype=E4M3)
+    if row_scale is None:
+        row_scale = torch.empty((rows,), device=x.device, dtype=torch.float32)
+    # the kernel stores eight codes at a time (8-byte aligned rows) and reads gamma / beta / pe as float4
+    if (out.dtype != E4M3 or out.device != x.device or out.stride(-1) != 1 or out.shape != (rows, C)
+            or out.data_ptr() % 8 or out.stride(0) % 8):
+        raise ValueError(f"out must be a [{rows}, {C}] float8_e4m3fn view on {x.device} with unit column stride and 8-byte "
+                         f"aligned rows, got {out.dtype} {tuple(out.shape)} strides {out.stride()} at offset {out.data_ptr() % 8}")
+    if row_scale.dtype != torch.float32 or row_scale.device != x.device or not row_scale.is_contiguous() \
+            or row_scale.numel() != rows:
+        raise ValueError(f"row_scale must be a contiguous fp32 [{rows}] vector on {x.device}")
+    for name, t, n in (("gamma", gamma, C), ("beta", beta, C), ("pe", pe, None)):
+        if t is None and name == "pe":
+            continue
+        if (t.dtype != torch.float32 or t.device != x.device or not t.is_contiguous() or t.data_ptr() % 16
+                or t.shape[-1] != C or (n is not None and t.numel() != n)):
+            raise ValueError(f"{name} must be contiguous fp32 on {x.device}, 16-byte aligned, with {C} columns; got "
+                             f"{t.dtype} {tuple(t.shape)} on {t.device}")
+    check(_ffi.lib().vx_layernorm_fp8(ptr(x), c_ll(x.stride(0)), c_ll(rows), c_int(C), ptr(gamma), ptr(beta),
+                                      c_float(eps), ptr(pe), c_int(rows_per_frame), c_int(0 if pe is None else pe.shape[0]),
+                                      ptr(out), c_ll(out.stride(0)), ptr(row_scale), stream_ptr()), "vx_layernorm_fp8")
+    return out, row_scale
 
 
 def geglu(x, out=None):
