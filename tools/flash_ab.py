@@ -1,12 +1,16 @@
 """A/B timing of the two flash-attention loops on the attention shapes of one UNet forward of the benchmark workload
 (b = 2 CFG halves x f = 16 frames, 64x64 latents, 8 heads).
 
-    python tools/flash_ab.py [--launches 50] [--rounds 3] [--plan]
+    python tools/flash_ab.py [--launches 50] [--rounds 3] [--baseline-lib LIB] [--plan]
 
-Per shape: old (VX_FA_V1=1, the serial loop) and new (default) alternate, A B A B, `--rounds` times each; one sample is
-`--launches` back-to-back launches between two CUDA events.  Prints ms per launch (median over rounds, with the spread),
-TFLOP/s by the benchmark's formula 4 B Nq Nk C, old / new, and for hd 40 the share of the exponential bound (a 64x64 score
-block costs a warpgroup 4096 ex2 at 16 per clock and SM = 256 clocks) at the SM clock sampled during the run.
+Per shape the arms alternate, A B (C) A B (C), `--rounds` times each:
+  old     VX_FA_V1=1, the serial loop of this build;
+  parent  (with --baseline-lib: a libvxb200.so built from an earlier commit) that library's default loop;
+  new     this build's default loop.
+One sample is `--launches` back-to-back launches between two CUDA events.  Prints ms per launch (median over rounds, with
+the spread), TFLOP/s by the benchmark's formula 4 B Nq Nk C, the speedup of new over old and over the parent, whether the
+outputs are bit-equal, and for hd 40 the share of the exponential bound (a 64x64 score block costs a warpgroup 4096 ex2 at
+16 per clock and SM = 256 clocks) at the SM clock sampled during the run.
 Inputs come from a seed.  `--plan` prints the shape and FLOP table and stops; timing without a CUDA device is an error."""
 import argparse
 import json
@@ -44,6 +48,7 @@ def main():
     ap.add_argument("--launches", type=int, default=50)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--plan", action="store_true")
+    ap.add_argument("--baseline-lib", default=None, help="libvxb200.so of an earlier build, timed as the parent arm")
     ap.add_argument("--json", default=None, help="also write the table to this file")
     args = ap.parse_args()
 
@@ -61,12 +66,21 @@ def main():
     print("device:", smi("name,power.limit,clocks.max.sm"))
     sms = torch.cuda.get_device_properties(0).multi_processor_count
 
-    def use_serial(on):
-        if on:
+    lib = _ffi.lib()
+    baseline = None
+    if args.baseline_lib:
+        import ctypes
+        baseline = ctypes.CDLL(os.path.abspath(args.baseline_lib))
+        baseline.vx_last_error.restype = ctypes.c_char_p
+    arms = ["old"] + (["parent"] if baseline is not None else []) + ["new"]
+
+    def use(arm):
+        if arm == "old":
             os.environ["VX_FA_V1"] = "1"
         else:
             os.environ.pop("VX_FA_V1", None)
-        _ffi.lib().vx_flash_reload_env()
+        _ffi._lib = baseline if arm == "parent" else lib
+        _ffi._lib.vx_flash_reload_env()
 
     rows = []
     for name, Bq, N, hd, kv_div in SHAPES:
@@ -77,18 +91,18 @@ def main():
         out = torch.empty_like(q)
         run = lambda: ops.flash_attention(q, kv[:, :C], kv[:, C:], HEADS, N, N, kv_div, out=out)
         results = {}
-        for serial in (True, False):
-            use_serial(serial)
+        for arm in arms:
+            use(arm)
             for _ in range(5):
                 run()
-            results[serial] = out.clone()
+            results[arm] = out.clone()
         torch.cuda.synchronize()
-        same = torch.equal(results[True], results[False])
-        ms = {True: [], False: []}
+        same = all(torch.equal(results["old"], r) for r in results.values())
+        ms = {arm: [] for arm in arms}
         clocks = []
         for _ in range(args.rounds):
-            for serial in (True, False):
-                use_serial(serial)
+            for arm in arms:
+                use(arm)
                 run()
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()
@@ -97,24 +111,31 @@ def main():
                 e1.record()
                 clk = smi("clocks.sm")   # sampled while the launches are in flight
                 e1.synchronize()
-                ms[serial].append(e0.elapsed_time(e1) / args.launches)
+                ms[arm].append(e0.elapsed_time(e1) / args.launches)
                 if clk.split()[0].isdigit():
                     clocks.append(int(clk.split()[0]))
-        use_serial(False)
+        use("new")
         med = {k: sorted(v)[len(v) // 2] for k, v in ms.items()}
         spread = {k: (max(v) - min(v)) / med[k] for k, v in ms.items()}
         mhz = sorted(clocks)[len(clocks) // 2] if clocks else None
-        row = {"shape": name.strip(), "Bq": Bq, "N": N, "hd": hd, "kv_div": kv_div, "bit_equal": same,
-               "old_ms": med[True], "new_ms": med[False], "old_spread": spread[True], "new_spread": spread[False],
-               "old_tflops": flops(Bq, N, hd) / med[True] / 1e9, "new_tflops": flops(Bq, N, hd) / med[False] / 1e9,
-               "speedup": med[True] / med[False], "sm_mhz": mhz}
-        line = (f"{name:14s} old {med[True]:8.4f} ms (+-{100 * spread[True]:4.1f}%) {row['old_tflops']:6.1f} TFLOP/s | "
-                f"new {med[False]:8.4f} ms (+-{100 * spread[False]:4.1f}%) {row['new_tflops']:6.1f} TFLOP/s | "
-                f"x{row['speedup']:.2f} | bit-equal {same} | SM {mhz} MHz")
+        row = {"shape": name.strip(), "Bq": Bq, "N": N, "hd": hd, "kv_div": kv_div, "bit_equal": same, "sm_mhz": mhz}
+        line = f"{name:14s}"
+        for arm in arms:
+            row[f"{arm}_ms"], row[f"{arm}_spread"] = med[arm], spread[arm]
+            row[f"{arm}_tflops"] = flops(Bq, N, hd) / med[arm] / 1e9
+            line += f" {arm} {med[arm]:8.4f} ms (+-{100 * spread[arm]:4.1f}%) {row[f'{arm}_tflops']:6.1f} TFLOP/s |"
+        row["speedup"] = med["old"] / med["new"]
+        line += f" new/old x{row['speedup']:.2f}"
+        if baseline is not None:
+            row["speedup_vs_parent"] = med["parent"] / med["new"]
+            line += f" new/parent x{row['speedup_vs_parent']:.2f}"
+        line += f" | bit-equal {same} | SM {mhz} MHz"
         if hd == 40 and mhz:
             bound = ex2_bound_ms(Bq, N, mhz, sms)
-            row["ex2_bound_share_old"], row["ex2_bound_share_new"] = bound / med[True], bound / med[False]
-            line += f" | ex2 bound {bound:.3f} ms: old {bound / med[True]:.2f}, new {bound / med[False]:.2f}"
+            line += " | ex2 bound " + f"{bound:.3f} ms:"
+            for arm in arms:
+                row[f"ex2_bound_share_{arm}"] = bound / med[arm]
+                line += f" {arm} {bound / med[arm]:.2f}"
         print(line, flush=True)
         rows.append(row)
     if args.json:

@@ -21,7 +21,8 @@
 // points (P -> bf16, O in fp32, O / l -> bf16), so their outputs are bit-identical:
 //   flash_attn_pipe_kernel  : one producer warp + NCONS consumer warpgroups (64 NCONS query rows per CTA) around a
 //                             full / empty mbarrier ring; each warpgroup issues S_{j+1} and O += P_j V_j together and
-//                             runs the softmax of S_{j+1} under the latter.  Serves hd <= kFaPipeMaxHd.
+//                             runs the softmax of S_{j+1} under the latter (at hd <= 56 with S_{j+2} also in flight,
+//                             two S register sets).  Serves hd <= 56, 80, 160.
 //   flash_attn_wgmma_kernel : one CTA = one warpgroup = 64 query rows, each step a serial chain.  Serves the wider
 //                             heads, and every head dim under VX_FA_V1=1 (the A/B reference).
 #include "vx_host.h"
@@ -194,11 +195,34 @@ flash_attn_wgmma_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_c
 // deliberate differences, neither visible in a result: exponentials are the bare ex2.approx.ftz (identical for every value
 // >= 2^-126; smaller ones, which vanish against l >= 1 and O in fp32, flush to zero), and O += P V runs at N = hd rather
 // than the padded width (m64n40k16 for hd 40), so V needs no padding chunk.
-constexpr int kFaPipeMaxHd = 56;   // hd 64 no longer fits the 104 registers a consumer gets with two CTAs per SM
-constexpr int kFaPipeStages = 4;
+//
+// Configuration per head width and consumer count.  A consumer thread holds O (HD / 2 floats), S (32 per register set)
+// and P (16 words):
+//   hd <= 56, three consumers : one CTA per SM, 24 / 160 registers (of the 128 x 4 that 512 threads launch with), two S
+//                               register sets (below)
+//   hd 80 / 160, two          : one CTA per SM, 24 / 232 (of 168 x 3), one S set
+//   one consumer (Nq <= 64)   : two CTAs per SM, 24 / 232 (of 128 x 2), one S set
+// and the ring is the deepest, up to 4 stages, that leaves room for that many CTAs.  Other widths take the serial loop.
+constexpr bool fa_pipe_hd(int hd) { return hd % 8 == 0 && (hd <= 56 || hd == 80 || hd == 160); }
+constexpr int fa_pipe_ncons(int hd, int Nq) { return Nq <= kFaRows ? 1 : hd <= 56 ? 3 : 2; }
+constexpr int fa_pipe_ctas(int ncons) { return ncons == 1 ? 2 : 1; }
+constexpr int fa_pipe_consumer_regs(int ncons) {
+  // what the launch allocates per thread (65536 / (CTAs x threads), in steps of 8), pooled over the warpgroups, less
+  // the producer's 24, shared among the consumers; setmaxnreg takes at most 232 (in steps of 8)
+  const int pool = 65536 / (fa_pipe_ctas(ncons) * 128 * (ncons + 1)) / 8 * 8 * (ncons + 1);
+  const int r = (pool - 24) / ncons / 8 * 8;
+  return r < 232 ? r : 232;
+}
+constexpr int fa_pipe_stages(int hd, int ncons) {
+  const int tile = kFaRows * ((hd + 15) / 16 * 16) * 2;
+  const int per_cta = 228 * 1024 / fa_pipe_ctas(ncons) - 1024 - 256;   // less the per-CTA reserve and barriers
+  const int s = (per_cta - ncons * tile) / (2 * tile);
+  return s < 4 ? s : 4;
+}
+static_assert(fa_pipe_stages(160, 1) >= 2 && fa_pipe_stages(160, 2) == 4 && fa_pipe_stages(56, 3) == 4, "ring depth");
 
 template <int HD, int NCONS>
-__global__ void __launch_bounds__(128 * (NCONS + 1), 2)
+__global__ void __launch_bounds__(128 * (NCONS + 1), fa_pipe_ctas(NCONS))
 flash_attn_pipe_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                        const __grid_constant__ CUtensorMap mapV, const FaArgs p) {
   constexpr int HDP = (HD + 15) / 16 * 16;   // Q / K tile width: the K dimension of S = Q K^T in steps of 16
@@ -235,7 +259,7 @@ flash_attn_pipe_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_co
   const int col_chunk = head * HD / 8;
   if (warp < 4) {
     // ------------------------------------------------------------------ producer (one lane)
-    if (NCONS == 2) setmaxnreg_dec<24>();   // 384 threads launch with 80 registers (two CTAs per SM): 24 + 2 x 104 <= 240
+    setmaxnreg_dec<24>();
     if (warp == 0 && lane == 0) {
       tma_prefetch_desc(&mapQ);
       tma_prefetch_desc(&mapK);
@@ -260,7 +284,7 @@ flash_attn_pipe_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_co
     return;
   }
   // -------------------------------------------------------------------- consumers
-  if (NCONS == 2) setmaxnreg_inc<104>();
+  setmaxnreg_inc<fa_pipe_consumer_regs(NCONS)>();
   const int wg = (warp >> 2) - 1;
   // Q / K: K-major, no swizzle: LBO = 64 rows x 16 B between the 8-wide head-dim chunks, SBO = 128 B between 8-row
   // groups; +2 chunks (+2048 B = +128 in the address field) per 16 head dims.
@@ -275,13 +299,13 @@ flash_attn_pipe_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_co
   for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, alpha[2];
 
-  auto issue_s = [&](int st) {   // S = Q K^T against stage st, one commit group
+  auto issue_s = [&](float (&s)[32], int st) {   // S = Q K^T against stage st, one commit group
     const uint64_t dk = make_smem_desc(smem_u32(sK + st * kTile), kFaRows * 16, 128, SWZ_NONE);
 #pragma unroll
     for (int k = 0; k < HDP / 16; ++k) Wgmma<64>::ss<0, 0>(s, dq + (uint64_t)(k * 128), dk + (uint64_t)(k * 128), k);
     wgmma_commit();
   };
-  auto softmax = [&](int j) {    // scores of step j in s -> alpha, m_run, l; s becomes the unrounded P
+  auto softmax = [&](float (&s)[32], int j) {    // scores of step j in s -> alpha, m_run, l; s becomes the unrounded P
     if ((j + 1) * kFaRows > p.Nk) {   // keys past Nk (the last, partial step) do not exist
 #pragma unroll
       for (int i = 0; i < 32; ++i)
@@ -309,19 +333,11 @@ flash_attn_pipe_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_co
       l[h] = i < 4 ? __fmaf_rn(l[h], alpha[h], e) : __fadd_rn(l[h], e);
     }
   };
-  auto pack = [&]() {            // P -> bf16, straight into the A fragments of O += P V
+  auto pack = [&](const float (&s)[32]) {   // P -> bf16, straight into the A fragments of O += P V
 #pragma unroll
     for (int i = 0; i < 32; i += 2) pa[i >> 3][(i >> 1) & 3] = pack_bf16(s[i], s[i + 1]);
   };
 
-  mbar_wait(q_full, 0);
-  mbar_wait(&kv_full[0], 0);
-  wgmma_fence();
-  issue_s(0);
-  wgmma_wait<0>();
-  wgmma_fence_regs(s);
-  softmax(0);
-  pack();
   auto issue_pv = [&](int st) {  // O += P V against stage st, one commit group
     const uint64_t dv = make_smem_desc(smem_u32(sV + st * kTile), 128, kFaRows * 16, SWZ_NONE);
 #pragma unroll
@@ -334,8 +350,92 @@ flash_attn_pipe_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_co
     for (int k = 0; k < 4; ++k) wgmma_fence_regs(pa[k]);
     if (lane == 0) mbar_arrive(&kv_empty[st]);
   };
+  auto rescale = [&]() {
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) o[i] = __fmul_rn(o[i], alpha[(i >> 1) & 1]);
+  };
+  mbar_wait(q_full, 0);
   int st = 0;
   uint32_t phase = 0;
+  if constexpr (NCONS == 3) {
+    // Two S register sets: S_{j+2} is issued behind O += P_j V_j and runs under the softmax of S_{j+1}, so no step waits
+    // for its own S = Q K^T.  Commit groups in issue order:
+    //   prologue   [S_0] [S_1]                 wait<1>  softmax(S_0) -> P_0
+    //   step j     [O += P_j V_j] [S_{j+2}]    wait<2>  S_{j+1} complete: softmax(S_{j+1})
+    //                                          wait<1>  O += P_j V_j complete: release stage j, O *= alpha, pack P_{j+1}
+    // and without S_{j+2} (j = T - 2) wait<1> / wait<0>.  The set S_{j+2} lands in held S_j, dead once P_j is packed.
+    float s2[32];
+    int ist = 0;              // stage / phase of the next S to issue
+    uint32_t iph = 0;
+    auto next_s = [&](float (&sx)[32]) {
+      mbar_wait(&kv_full[ist], iph);
+      wgmma_fence();
+      issue_s(sx, ist);
+      if (++ist == p.stages) {
+        ist = 0;
+        iph ^= 1;
+      }
+    };
+    // Every path through the loop reaches each wait with the same groups in flight (ptxas serialises every wgmma of the
+    // kernel when it cannot prove that): one consumer step per tail shape, T = 1 apart.
+    auto step = [&](float (&cur)[32], float (&nxt)[32], int j) {   // P_j in pa, S_{j+1} in flight into cur
+      wgmma_fence();
+      issue_pv(st);
+      next_s(nxt);
+      wgmma_wait<2>();
+      wgmma_fence_regs(cur);
+      softmax(cur, j + 1);
+      wgmma_wait<1>();
+      pv_done(st);
+      rescale();
+      pack(cur);
+      if (++st == p.stages) st = 0;
+    };
+    auto last = [&](float (&cur)[32], int j) {   // j = T - 2: no S_{j+2}
+      wgmma_fence();
+      issue_pv(st);
+      wgmma_wait<1>();
+      wgmma_fence_regs(cur);
+      softmax(cur, j + 1);
+      wgmma_wait<0>();
+      pv_done(st);
+      rescale();
+      pack(cur);
+      if (++st == p.stages) st = 0;
+    };
+    next_s(s);
+    if (T == 1) {
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      softmax(s, 0);
+      pack(s);
+    } else {
+      next_s(s2);
+      wgmma_wait<1>();
+      wgmma_fence_regs(s);
+      softmax(s, 0);
+      pack(s);
+      for (int j = 0;; j += 2) {   // S_{j+1} in flight into s2
+        if (j + 2 >= T) {
+          last(s2, j);
+          break;
+        }
+        step(s2, s, j);
+        if (j + 3 >= T) {
+          last(s, j + 1);
+          break;
+        }
+        step(s, s2, j + 1);
+      }
+    }
+  } else {
+  mbar_wait(&kv_full[0], 0);
+  wgmma_fence();
+  issue_s(s, 0);
+  wgmma_wait<0>();
+  wgmma_fence_regs(s);
+  softmax(s, 0);
+  pack(s);
   for (int j = 0; j + 1 < T; ++j) {
     int st1 = st + 1;
     uint32_t phase1 = phase;
@@ -345,18 +445,18 @@ flash_attn_pipe_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_co
     }
     mbar_wait(&kv_full[st1], phase1);
     wgmma_fence();
-    issue_s(st1);
+    issue_s(s, st1);
     issue_pv(st);
     wgmma_wait<1>();
     wgmma_fence_regs(s);
-    softmax(j + 1);
+    softmax(s, j + 1);
     wgmma_wait<0>();
     pv_done(st);
-#pragma unroll
-    for (int i = 0; i < HD / 2; ++i) o[i] = __fmul_rn(o[i], alpha[(i >> 1) & 1]);
-    pack();
+    rescale();
+    pack(s);
     st = st1;
     phase = phase1;
+  }
   }
   wgmma_fence();
   issue_pv(st);   // the last step has no successor to overlap
@@ -479,11 +579,11 @@ extern "C" int vx_flash_attention(const void* q, long long ldq, const void* k, l
     return 0;
   }
   const int hdp = (hd + 15) / 16 * 16;
-  const bool pipe = hd <= kFaPipeMaxHd && !fa_v1();
-  // query rows per CTA: two consumer warpgroups, one where a single 64-row tile covers the frame
-  const int ncons = pipe && Nq > kFaRows ? 2 : 1;
+  const bool pipe = fa_pipe_hd(hd) && !fa_v1();
+  // query rows per CTA: 64 per consumer warpgroup (fa_pipe_ncons)
+  const int ncons = pipe ? fa_pipe_ncons(hd, Nq) : 1;
   // K / V ring depth of the serial loop: two stages for the wide heads keep two CTAs per SM resident, three otherwise
-  const int stages = pipe ? kFaPipeStages : hdp > 96 ? 2 : 3;
+  const int stages = pipe ? fa_pipe_stages(hd, ncons) : hdp > 96 ? 2 : 3;
   const size_t smem = (size_t)(ncons + 2 * stages) * kFaRows * hdp * 2 + 128 + 128;
   CUtensorMap mQ, mK, mV;
   const void* ptrs[3] = {q, k, v};
@@ -507,10 +607,13 @@ extern "C" int vx_flash_attention(const void* q, long long ldq, const void* k, l
     switch (hd) {
 #define VX_FA_CASE(H)                                                                                       \
     case H:                                                                                                 \
-      if (ncons == 2) e = launch_fa<flash_attn_pipe_kernel<H, 2>>(grid, 384, smem, cs, mQ, mK, mV, a);         \
+      if (ncons == fa_pipe_ncons(H, kFaRows + 1))                                                           \
+        e = launch_fa<flash_attn_pipe_kernel<H, fa_pipe_ncons(H, kFaRows + 1)>>(grid, 128 * (ncons + 1), smem, cs, mQ, \
+                                                                             mK, mV, a);                 \
       else e = launch_fa<flash_attn_pipe_kernel<H, 1>>(grid, 256, smem, cs, mQ, mK, mV, a);                    \
       break;
       VX_FA_CASE(8) VX_FA_CASE(16) VX_FA_CASE(24) VX_FA_CASE(32) VX_FA_CASE(40) VX_FA_CASE(48) VX_FA_CASE(56)
+      VX_FA_CASE(80) VX_FA_CASE(160)
 #undef VX_FA_CASE
       default: return fail("vx_flash_attention: hd=%d unsupported", hd);
     }
