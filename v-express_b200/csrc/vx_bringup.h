@@ -14,6 +14,7 @@ int vx_probe_tma(const void* base, int rank, const unsigned long long* dims, con
 
 void vx_flash_reload_env(void);
 void vx_gemm_reload_env(void);
+void vx_norm_reload_env(void);
 void vx_pdl_set(int on);   /* programmatic dependent launch on / off (default: VX_PDL, read once) */
 int vx_pdl_get(void);
 #ifdef __cplusplus

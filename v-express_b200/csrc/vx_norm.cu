@@ -54,18 +54,32 @@ struct GnStatsArgs {
   float* partial;
 };
 
+// The statistics are sums of x - pivot, pivot = the bf16 value at pixel 0 of the group's first channel in frame n: the
+// same value for every chunk, CTA and kernel, so partials (whose means are relative to it) merge as before.  Without the
+// shift, fp32 sums of x and x^2 cancel in M2 = sum x^2 - mean sum x once a group's mean is large against its spread (the
+// relative variance error grows as (mean / std)^2); with it, x - pivot is exact in fp32 and of the size of the spread.
+__device__ __forceinline__ float gn_pivot(const __nv_bfloat16* x1, long long ld1, int C1, const __nv_bfloat16* x2,
+                                          long long ld2, int HW, int n, int g, int cpg) {
+  const int c = g * cpg;
+  return __bfloat162float(c < C1 ? x1[(long long)n * HW * ld1 + c] : x2[(long long)n * HW * ld2 + (c - C1)]);
+}
+
 __device__ __forceinline__ void gn_stats_body(const GnStatsArgs& p, float* sm, const int n, const int s) {
   // sm: [R][C] sums, [R][C] sumsq
   const int C = p.C1 + p.C2;
   const int V = C / 8;
+  const int cpg = C / p.G;
   const int v = threadIdx.x % V, r = threadIdx.x / V;
   const int chunk = (p.HW + p.S - 1) / p.S;
   const int p0 = s * chunk;
   const int p1 = min(p.HW, p0 + chunk);
-  float sum[8], sq[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) sum[i] = sq[i] = 0.f;
+  float sum[8], sq[8], piv[8];
   const int c0 = v * 8;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    sum[i] = sq[i] = 0.f;
+    piv[i] = gn_pivot(p.x1, p.ld1, p.C1, p.x2, p.ld2, p.HW, n, (c0 + i) / cpg, cpg);   // independent loads, L1 hits
+  }
   const bool second = c0 >= p.C1;
   const __nv_bfloat16* base = second ? p.x2 + (long long)n * p.HW * p.ld2 + (c0 - p.C1)
                                      : p.x1 + (long long)n * p.HW * p.ld1 + c0;
@@ -76,8 +90,9 @@ __device__ __forceinline__ void gn_stats_body(const GnStatsArgs& p, float* sm, c
     load8(base + px * ld, f);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      sum[i] += f[i];
-      sq[i] += f[i] * f[i];
+      const float d = f[i] - piv[i];
+      sum[i] += d;
+      sq[i] += d * d;
     }
   }
   float* ssum = sm;
@@ -88,8 +103,7 @@ __device__ __forceinline__ void gn_stats_body(const GnStatsArgs& p, float* sm, c
     ssq[r * C + c0 + i] = sq[i];
   }
   __syncthreads();
-  const int cpg = C / p.G;
-  for (int g = threadIdx.x; g < p.G; g += blockDim.x) {
+  for (int g = threadIdx.x; g < p.G; g += blockDim.x) {   // mean relative to the group's pivot
     float a = 0.f, b = 0.f;
     for (int rr = 0; rr < p.R; ++rr)
       for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
@@ -124,6 +138,16 @@ struct GnApplyArgs {
   int chunk;  // pixels per CTA
 };
 
+// SiLU as y sigmoid(y), sigmoid(y) = 0.5 + 0.5 tanh(y / 2): one MUFU op per element.  tanh.approx is within a relative
+// 2^-11 of tanh, so sigmoid is within 2^-12 absolute: on the negative tail (y < -4) that is more than the bf16 rounding of
+// silu(y).  __fdividef(y, 1 + __expf(-y)) is accurate to a few 2^-23 there but took up to 1.38x the kernel time (1.28x
+// summed over the VAE decoder's shapes) on an H100 SXM at 700 W (tools/norm_ab_h100.txt).
+__device__ __forceinline__ float gn_silu(float y) {
+  float t;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * y));
+  return y * fmaf(0.5f, t, 0.5f);
+}
+
 // `depart` (fused kernel only): called by every thread once the partial statistics of the frame have been merged, i.e.
 // when this CTA no longer depends on its peers.
 template <typename Depart>
@@ -134,6 +158,9 @@ __device__ __forceinline__ void gn_apply_body(const GnApplyArgs& p, float* sm, c
   float* shift = sm + C;
   float* gmean = sm + 2 * C;
   float* grstd = gmean + p.G;
+  const int cpg = C / p.G;
+  // the pivot of group threadIdx.x (the partial means are relative to it, gn_stats_body), in flight during the merge
+  const float gpiv = (int)threadIdx.x < p.G ? gn_pivot(p.x1, p.ld1, p.C1, p.x2, p.ld2, p.HW, n, threadIdx.x, cpg) : 0.f;
   {
     // Chan et al. parallel-variance merge of the S partials of every group: one warp per group, lane s holds partial
     // s (and s + 32), then a fixed shuffle-down tree -- the same order in every CTA and every run (deterministic).
@@ -172,7 +199,9 @@ __device__ __forceinline__ void gn_apply_body(const GnApplyArgs& p, float* sm, c
   }
   __syncthreads();
   depart();
-  const int cpg = C / p.G;
+  for (int g = threadIdx.x; g < p.G; g += blockDim.x)
+    gmean[g] += g == (int)threadIdx.x ? gpiv : gn_pivot(p.x1, p.ld1, p.C1, p.x2, p.ld2, p.HW, n, g, cpg);
+  __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const int g = c / cpg;
     const float sc = grstd[g] * p.gamma[c];
@@ -214,14 +243,8 @@ __device__ __forceinline__ void gn_apply_body(const GnApplyArgs& p, float* sm, c
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      float y = fmaf(f[i], sc[i], sh[i]);
-      if (p.silu) {
-        // y * sigmoid(y) with sigmoid(y) = 0.5 + 0.5 * tanh(y / 2): one MUFU op per element
-        float t;
-        asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * y));
-        y = y * fmaf(0.5f, t, 0.5f);
-      }
-      f[i] = y;
+      const float y = fmaf(f[i], sc[i], sh[i]);
+      f[i] = p.silu ? gn_silu(y) : y;
     }
     __stcs(reinterpret_cast<uint4*>(dst + (long long)px * p.ldo),
            make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7])));
@@ -317,7 +340,9 @@ __device__ __forceinline__ float gn_ld_dsmem(const float* local, uint32_t rank) 
   return v;
 }
 
-__global__ void gn_cluster_kernel(const GnClusterArgs p) {
+// At most 640 threads (R = 640 / V pixel lanes, C <= GN_MAX_C) and <= 48 registers, i.e. two CTAs per SM: at the 54
+// registers the pivots take without the cap, the 8x8 level (32 frames, clusters of four) took 1.5x the time.
+__global__ void __launch_bounds__(640, 2) gn_cluster_kernel(const GnClusterArgs p) {
   pdl_enter();
   extern __shared__ __align__(16) uint8_t gn_smem[];
   const int C = p.C1 + p.C2, V = C / 8, G = p.G, cpg = C / G, R = p.R, P = p.P;
@@ -338,9 +363,12 @@ __global__ void gn_cluster_kernel(const GnClusterArgs p) {
   const __nv_bfloat16* base = second ? p.x2 + (long long)n * p.HW * p.ld2 + (c0 - p.C1)
                                      : p.x1 + (long long)n * p.HW * p.ld1 + c0;
   const long long ld = second ? p.ld2 : p.ld1;
-  float sum[8], sq[8];
+  float sum[8], sq[8], piv[8];   // sums of x - pivot (gn_stats_body)
 #pragma unroll
-  for (int i = 0; i < 8; ++i) sum[i] = sq[i] = 0.f;
+  for (int i = 0; i < 8; ++i) {
+    sum[i] = sq[i] = 0.f;
+    piv[i] = gn_pivot(p.x1, p.ld1, p.C1, p.x2, p.ld2, p.HW, n, (c0 + i) / cpg, cpg);
+  }
   constexpr int U = 4;   // global loads in flight per thread
   int px = r;
   for (; px + (U - 1) * R < P; px += U * R) {
@@ -354,8 +382,9 @@ __global__ void gn_cluster_kernel(const GnClusterArgs p) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float2 t = unpack_bf16(w4[i]);
-        sum[2 * i] += t.x; sq[2 * i] = fmaf(t.x, t.x, sq[2 * i]);
-        sum[2 * i + 1] += t.y; sq[2 * i + 1] = fmaf(t.y, t.y, sq[2 * i + 1]);
+        const float d0 = t.x - piv[2 * i], d1 = t.y - piv[2 * i + 1];
+        sum[2 * i] += d0; sq[2 * i] = fmaf(d0, d0, sq[2 * i]);
+        sum[2 * i + 1] += d1; sq[2 * i + 1] = fmaf(d1, d1, sq[2 * i + 1]);
       }
     }
   }
@@ -366,8 +395,9 @@ __global__ void gn_cluster_kernel(const GnClusterArgs p) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float2 t = unpack_bf16(w4[i]);
-      sum[2 * i] += t.x; sq[2 * i] = fmaf(t.x, t.x, sq[2 * i]);
-      sum[2 * i + 1] += t.y; sq[2 * i + 1] = fmaf(t.y, t.y, sq[2 * i + 1]);
+      const float d0 = t.x - piv[2 * i], d1 = t.y - piv[2 * i + 1];
+      sum[2 * i] += d0; sq[2 * i] = fmaf(d0, d0, sq[2 * i]);
+      sum[2 * i + 1] += d1; sq[2 * i + 1] = fmaf(d1, d1, sq[2 * i + 1]);
     }
   }
 #pragma unroll
@@ -399,7 +429,7 @@ __global__ void gn_cluster_kernel(const GnClusterArgs p) {
       m2 += qb + delta * delta * (cnt * cb / tot);
       cnt = tot;
     }
-    gmean[g] = mean;
+    gmean[g] = gn_pivot(p.x1, p.ld1, p.C1, p.x2, p.ld2, p.HW, n, g, cpg) + mean;   // one load per group, in parallel
     grstd[g] = rsqrtf(m2 / cnt + p.eps);
   }
   __syncthreads();
@@ -429,13 +459,8 @@ __global__ void gn_cluster_kernel(const GnClusterArgs p) {
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      float y = fmaf(f[i], sc[i], sh[i]);
-      if (p.silu) {
-        float t;
-        asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * y));
-        y = y * fmaf(0.5f, t, 0.5f);
-      }
-      f[i] = y;
+      const float y = fmaf(f[i], sc[i], sh[i]);
+      f[i] = p.silu ? gn_silu(y) : y;
     }
     store8(dst + (long long)(p0 + q) * p.ldo, f);
   }
@@ -807,9 +832,15 @@ __global__ void row_stats_kernel(const __nv_bfloat16* __restrict__ x, long long 
 
 using namespace vx;
 
+// Every kernel in this file moves 16-byte vectors (8 bf16 / 4 fp32 values) and never checks the address: the entry points
+// reject pointers and leading dimensions that would make one of them misaligned, before any CUDA call.
+static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
 extern "C" int vx_softmax_rows(const float* x, long long ldx, long long rows, int n, void* out, long long ldo,
                                void* stream) {
-  VX_REQUIRE(n % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0, "vx_softmax_rows: n=%d must be a multiple of 4", n);
+  VX_REQUIRE(al16(x) && al16(out) && ldx % 4 == 0 && ldo % 4 == 0,
+             "vx_softmax_rows: x / out must be 16-byte aligned and ldx=%lld, ldo=%lld multiples of 4", ldx, ldo);
+  VX_REQUIRE(n % 4 == 0, "vx_softmax_rows: n=%d must be a multiple of 4", n);
   launch_k(softmax_rows_kernel, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream, x, ldx, n, (__nv_bfloat16*)out, ldo);
   VX_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -826,12 +857,26 @@ static int gn_block(int C, int* R) {
 
 extern "C" int vx_groupnorm_stats_ws_floats(int NB, int G, int S) { return NB * S * G * 3; }
 
+// Widest [x1 | x2]: the apply and one-launch kernels run C / 8 threads for C >= 2048, and at their ~80 registers a
+// 1024-thread block (C = 8192) does not fit the register file.  The model's widest GroupNorm is 2560.
+constexpr int GN_MAX_C = 4096;
+
+// [x1 | x2] (x2 only when C2 > 0) and out (when given) 16-byte aligned, leading dimensions multiples of 8
+static bool gn_layout_ok(const void* x1, long long ld1, const void* x2, long long ld2, int C2, const void* out, long long ldo) {
+  return al16(x1) && ld1 % 8 == 0 && (C2 == 0 || (al16(x2) && ld2 % 8 == 0)) && al16(out) && ldo % 8 == 0;
+}
+#define GN_REQUIRE_LAYOUT(name, out, ldo)                                                                          \
+  VX_REQUIRE(gn_layout_ok(x1, ld1, x2, ld2, C2, out, ldo),                                                          \
+             "%s: x1 / x2 / out must be 16-byte aligned with leading dimensions multiples of 8 (ld1=%lld ld2=%lld ldo=%lld)", \
+             name, ld1, ld2, (long long)(ldo))
+
 // x = [x1 | x2] per row (x2 may be null, C2 = 0); rows = NB*HW; partial: float[NB*S*G*3] workspace.
 extern "C" int vx_groupnorm_stats(const void* x1, long long ld1, int C1, const void* x2, long long ld2, int C2,
                                   int NB, int HW, int G, int S, float* partial, void* stream) {
+  GN_REQUIRE_LAYOUT("vx_groupnorm_stats", nullptr, 0);
   const int C = C1 + C2;
   VX_REQUIRE(C1 % 8 == 0 && C2 % 8 == 0 && C % G == 0 && S >= 1, "vx_groupnorm_stats: bad C1=%d C2=%d G=%d", C1, C2, G);
-  VX_REQUIRE(C / 8 <= 1024, "vx_groupnorm_stats: C=%d too wide", C);
+  VX_REQUIRE(C <= GN_MAX_C, "vx_groupnorm_stats: C=%d too wide (at most %d)", C, GN_MAX_C);
   GnStatsArgs a{(const __nv_bfloat16*)x1, ld1, C1, (const __nv_bfloat16*)x2, ld2, C2, HW, G, S, 0, partial};
   const int threads = gn_block(C, &a.R);
   const size_t smem = (size_t)2 * a.R * C * sizeof(float);
@@ -846,8 +891,10 @@ extern "C" int vx_groupnorm_stats(const void* x1, long long ld1, int C1, const v
 extern "C" int vx_groupnorm_apply(const void* x1, long long ld1, int C1, const void* x2, long long ld2, int C2,
                                   int NB, int HW, int G, int S, const float* partial, const float* gamma,
                                   const float* beta, float eps, int silu, void* out, long long ldo, void* stream) {
+  GN_REQUIRE_LAYOUT("vx_groupnorm_apply", out, ldo);
   const int C = C1 + C2;
   VX_REQUIRE(C1 % 8 == 0 && C2 % 8 == 0 && C % G == 0, "vx_groupnorm_apply: bad C1=%d C2=%d G=%d", C1, C2, G);
+  VX_REQUIRE(C <= GN_MAX_C, "vx_groupnorm_apply: C=%d too wide (at most %d)", C, GN_MAX_C);
   GnApplyArgs a{(const __nv_bfloat16*)x1, ld1, C1, (const __nv_bfloat16*)x2, ld2, C2, HW, G, S, partial, gamma, beta,
                 eps, silu, (__nv_bfloat16*)out, ldo, 0};
   VX_REQUIRE(S >= 1, "vx_groupnorm_apply: S=%d", S);
@@ -889,9 +936,10 @@ extern "C" int vx_groupnorm_capacity(int C) {
 extern "C" int vx_groupnorm_fused(const void* x1, long long ld1, int C1, const void* x2, long long ld2, int C2, int NB,
                                   int HW, int G, int S, float* partial, int* counters, const float* gamma,
                                   const float* beta, float eps, int silu, void* out, long long ldo, void* stream) {
+  GN_REQUIRE_LAYOUT("vx_groupnorm_fused", out, ldo);
   const int C = C1 + C2;
   VX_REQUIRE(C1 % 8 == 0 && C2 % 8 == 0 && C % G == 0 && S >= 1, "vx_groupnorm_fused: bad C1=%d C2=%d G=%d", C1, C2, G);
-  VX_REQUIRE(C / 8 <= 1024 && counters, "vx_groupnorm_fused: C=%d too wide / no counters", C);
+  VX_REQUIRE(C <= GN_MAX_C && counters, "vx_groupnorm_fused: C=%d too wide (at most %d) / no counters", C, GN_MAX_C);
   GnFusedArgs a{};
   a.st = GnStatsArgs{(const __nv_bfloat16*)x1, ld1, C1, (const __nv_bfloat16*)x2, ld2, C2, HW, G, S, 0, partial};
   const int threads = gn_block(C, &a.st.R);
@@ -925,8 +973,10 @@ extern "C" int vx_groupnorm_fused(const void* x1, long long ld1, int C1, const v
 extern "C" int vx_groupnorm_cluster(const void* x1, long long ld1, int C1, const void* x2, long long ld2, int C2, int NB,
                                     int HW, int G, const float* gamma, const float* beta, float eps, int silu, void* out,
                                     long long ldo, void* stream) {
+  GN_REQUIRE_LAYOUT("vx_groupnorm_cluster", out, ldo);
   const int C = C1 + C2;
-  VX_REQUIRE(C1 % 8 == 0 && C2 % 8 == 0 && C % G == 0 && C / 8 <= 1024, "vx_groupnorm_cluster: bad C1=%d C2=%d G=%d", C1, C2, G);
+  VX_REQUIRE(C1 % 8 == 0 && C2 % 8 == 0 && C % G == 0, "vx_groupnorm_cluster: bad C1=%d C2=%d G=%d", C1, C2, G);
+  VX_REQUIRE(C <= GN_MAX_C, "vx_groupnorm_cluster: C=%d too wide (at most %d)", C, GN_MAX_C);
   const int V = C / 8;
   int R = 640 / V;                       // ~640 threads: 4 pixel lanes at C = 1280, 2 at C = 2560
   if (R < 1) R = 1;
@@ -974,6 +1024,14 @@ extern "C" int vx_groupnorm_cluster(const void* x1, long long ld1, int C1, const
   return 0;
 }
 
+// VX_LN_V1: every C on the one-warp-per-row layernorm_kernel (A/B switch, read once; tests that compare the two kernels in
+// one process re-read it through vx_norm_reload_env).
+static bool& ln_v1() {
+  static bool v = getenv("VX_LN_V1") != nullptr;
+  return v;
+}
+extern "C" void vx_norm_reload_env() { ln_v1() = getenv("VX_LN_V1") != nullptr; }
+
 // pe: optional float [pe_frames, C]; row r uses pe[(r / rows_per_frame) % pe_frames].  TOut = uint8_t: e4m3 codes + row_scale.
 template <typename TOut>
 static int layernorm_entry(const void* x, long long ldx, long long rows, int C, const float* gamma, const float* beta,
@@ -981,8 +1039,13 @@ static int layernorm_entry(const void* x, long long ldx, long long rows, int C, 
                            float* row_scale, void* stream) {
   constexpr bool F8 = sizeof(TOut) == 1;
   const char* name = F8 ? "vx_layernorm_fp8" : "vx_layernorm";
+  // x: 16-byte rows; gamma / beta / pe: float4 loads; out: 16-byte (bf16) or 8-byte (e4m3) stores
+  VX_REQUIRE(al16(x) && ldx % 8 == 0 && ((uintptr_t)out & (F8 ? 7 : 15)) == 0 && ldo % 8 == 0 && al16(gamma) && al16(beta) &&
+                 al16(pe),
+             "%s: x / gamma / beta / pe must be 16-byte aligned, out %d-byte aligned, ldx=%lld and ldo=%lld multiples of 8",
+             name, F8 ? 8 : 16, ldx, ldo);
   VX_REQUIRE(C % 8 == 0 && C <= 2048, "%s: C=%d unsupported", name, C);
-  VX_REQUIRE(!F8 || (row_scale && ldo % 8 == 0), "vx_layernorm_fp8: row_scale missing or ldo %% 8 != 0");
+  VX_REQUIRE(!F8 || row_scale, "vx_layernorm_fp8: row_scale missing");
   const int threads = 256;
   const long long blocks = (rows * 32 + threads - 1) / threads;
   const int V = C / 8;
@@ -990,9 +1053,8 @@ static int layernorm_entry(const void* x, long long ldx, long long rows, int C, 
   if (pe && (rows_per_frame <= 0 || pe_frames <= 0)) return fail("%s: bad pe args", name);
   // The positional-encoding variant (temporal attention norms) takes the same kernel since its parameters moved to shared
   // memory: 63.5 -> ~41 us at the 320-wide level (the one-warp-per-row kernel used to be as fast).  VX_LN_PE5=0: old choice.
-  static const bool ln_v1 = getenv("VX_LN_V1") != nullptr;   // A/B switch, read once
   static const bool ln_pe5 = !(getenv("VX_LN_PE5") && atoi(getenv("VX_LN_PE5")) == 0);
-  if ((C == 320 || C == 640 || C == 1280) && (!pe || ln_pe5) && ldx % 8 == 0 && ldo % 8 == 0 && !ln_v1) {
+  if ((C == 320 || C == 640 || C == 1280) && (!pe || ln_pe5) && !ln_v1()) {
     const int lpr = C / 40;
     const long long groups = (rows + 32 / lpr - 1) / (32 / lpr);
     long long nb = ((groups + 1) / 2 + 7) / 8;
@@ -1050,6 +1112,8 @@ extern "C" int vx_layernorm_fp8(const void* x, long long ldx, long long rows, in
 // x: [rows, 2*inner] = (h | gate) -> out [rows, inner]
 extern "C" int vx_geglu(const void* x, long long ldx, long long rows, int inner, void* out, long long ldo,
                         void* stream) {
+  VX_REQUIRE(al16(x) && al16(out) && ldx % 8 == 0 && ldo % 8 == 0,
+             "vx_geglu: x / out must be 16-byte aligned and ldx=%lld, ldo=%lld multiples of 8", ldx, ldo);
   VX_REQUIRE(inner % 8 == 0, "vx_geglu: inner=%d", inner);
   const long long total = rows * (inner / 8);
   long long blocks = (total + 255) / 256;
@@ -1063,7 +1127,9 @@ extern "C" int vx_geglu(const void* x, long long ldx, long long rows, int inner,
 
 // stats: float[rows][2] = (mean, rstd) of every row of x (LayerNorm statistics, eps inside the rsqrt like torch)
 extern "C" int vx_row_stats(const void* x, long long ldx, long long rows, int C, float eps, float* stats, void* stream) {
-  VX_REQUIRE(C % 8 == 0 && C <= 2048 && ldx % 8 == 0, "vx_row_stats: C=%d unsupported", C);
+  VX_REQUIRE(al16(x) && ldx % 8 == 0 && ((uintptr_t)stats & 7) == 0,
+             "vx_row_stats: x must be 16-byte aligned with ldx=%lld a multiple of 8, stats 8-byte aligned", ldx);
+  VX_REQUIRE(C % 8 == 0 && C <= 2048, "vx_row_stats: C=%d unsupported", C);
   auto st = (cudaStream_t)stream;
   if (C == 320 || C == 640 || C == 1280) {
     const int lpr = C / 40;

@@ -20,6 +20,16 @@ def _chk_bf16(*ts):
             assert t.is_cuda and t.dtype == BF16 and t.stride(-1) == 1, (t.dtype, t.device, t.stride())
 
 
+def _chk_vectors(what, ld_mult, *ts):
+    """The norm / activation kernels move 16-byte vectors and never check an address: every tensor handed to them must
+    start 16-byte aligned and (2-D) have a row stride that is a multiple of ``ld_mult`` elements (8 bf16, 4 fp32)."""
+    for t in ts:
+        if t is not None and (t.data_ptr() % 16 or (t.dim() == 2 and t.stride(0) % ld_mult)):
+            raise ValueError(f"{what}: operands must be 16-byte aligned with row strides that are multiples of {ld_mult}, "
+                             f"got a {tuple(t.shape)} {t.dtype} view at byte offset {t.data_ptr() % 16} (mod 16), "
+                             f"strides {t.stride()}")
+
+
 def _chk_bias(bias, N, device, bias2=None, M=1, bias2_div=1):
     """The epilogue reads bias[n] and bias2[(m // bias2_div) * N + n] (n < N, m < M) as float2 from raw pointers: both must
     be fp32 on the output's device with unit column stride and 8-byte alignment, bias N entries, bias2 N columns and
@@ -151,6 +161,7 @@ def gemm_fp8(a, a_scale, w, w_scale, bias=None, *, bias2=None, bias2_div=1, scal
 # ---- LayerNorm folded into the consumer GEMM (experiment; the engine uses it only under VX_LN_FOLD=1)
 def row_stats(x, eps=1e-5, out=None):
     """(mean, rstd) of every row of x [rows, C] bf16 -> fp32 [rows, 2]."""
+    _chk_vectors("row_stats", 8, x)
     _chk_bf16(x)
     rows, C = x.shape
     if out is None:
@@ -454,6 +465,7 @@ def groupnorm(x1, NB, HW, gamma, beta, eps, silu, x2=None, groups=32, out=None, 
     grp = int(os.environ.get("VX_GN_FRAMES", "0"))
     if 0 < grp < NB:
         return _groupnorm_grouped(x1, NB, HW, gamma, beta, eps, silu, x2, groups, out, grp)
+    _chk_vectors("groupnorm", 8, x1, x2, out)
     _chk_bf16(x1, x2, out)
     C1 = x1.shape[1]
     C2 = 0 if x2 is None else x2.shape[1]
@@ -487,6 +499,7 @@ def groupnorm(x1, NB, HW, gamma, beta, eps, silu, x2=None, groups=32, out=None, 
 
 
 def _groupnorm_grouped(x1, NB, HW, gamma, beta, eps, silu, x2, groups, out, grp):
+    _chk_vectors("groupnorm", 8, x1, x2, out)
     _chk_bf16(x1, x2, out)
     C1 = x1.shape[1]
     C2 = 0 if x2 is None else x2.shape[1]
@@ -511,6 +524,7 @@ def _groupnorm_grouped(x1, NB, HW, gamma, beta, eps, silu, x2, groups, out, grp)
 
 
 def layernorm(x, gamma, beta, eps=1e-5, pe=None, rows_per_frame=0, out=None):
+    _chk_vectors("layernorm", 8, x, out, gamma, beta, pe)
     _chk_bf16(x, out)
     rows, C = x.shape
     if out is None:
@@ -524,6 +538,7 @@ def layernorm(x, gamma, beta, eps=1e-5, pe=None, rows_per_frame=0, out=None):
 def layernorm_fp8(x, gamma, beta, eps=1e-5, pe=None, rows_per_frame=0, out=None, row_scale=None):
     """layernorm() as the A operand of gemm_fp8: (float8_e4m3fn codes [rows, C], fp32 row_scale [rows]) with
     codes * row_scale ~ LayerNorm(x) [+ pe] computed in fp32, row_scale = amax(|row|) / 448 (1 for an all-zero row)."""
+    _chk_vectors("layernorm_fp8", 8, x)
     _chk_bf16(x)
     rows, C = x.shape
     if out is None:
@@ -552,6 +567,7 @@ def layernorm_fp8(x, gamma, beta, eps=1e-5, pe=None, rows_per_frame=0, out=None,
 
 
 def geglu(x, out=None):
+    _chk_vectors("geglu", 8, x, out)
     _chk_bf16(x, out)
     rows, two = x.shape
     inner = two // 2
@@ -649,6 +665,7 @@ def ddim_step(latents, acc, sqrt_a, sqrt_1ma, sqrt_aprev, sqrt_1maprev):
 
 def softmax_rows(x, out=None):
     """Row softmax of fp32 scores [rows, n] -> bf16 probabilities."""
+    _chk_vectors("softmax_rows", 4, x, out)
     assert x.dtype == torch.float32 and x.stride(1) == 1
     rows, n = x.shape
     if out is None:
