@@ -190,14 +190,17 @@ def geglu_ref64(a, w, bias):
         G, _, Pg = linear_ref64(a[r0:r1], w[inner:], bias[inner:])
         dV = K * 2.0 ** -22 * Pv + 2.0 ** -22 * (Pv + bias[:inner].double().abs())
         dG = K * 2.0 ** -22 * Pg + 2.0 ** -22 * (Pg + bias[inner:].double().abs())
-        gl = _gelu64(G)
-        dgelu = (0.5 * (1 + torch.erf(G / math.sqrt(2))) + G * torch.exp(-0.5 * G * G) / math.sqrt(2 * math.pi)).abs()
-        d1 = torch.clamp(dgelu + 0.8 * dG, max=1.13)
-        e_gelu = G.abs() * (2.0 ** -22 + 2.0 ** -18 * torch.erfc(G.abs() / math.sqrt(2))) + 2.0 ** -21 * gl.abs()
-        ref[r0:r1] = V * gl
-        bnd[r0:r1] = (gl.abs() * dV + V.abs() * (d1 * dG + e_gelu) + dV * (1.13 * dG + e_gelu)
-                      + 2.0 ** -22 * (V * gl).abs())
+        ref[r0:r1], bnd[r0:r1] = geglu_propagate(V, G, dV, dG)
     return ref, bnd
+
+
+def geglu_propagate(V, G, dV, dG):
+    """(V gelu(G), bound without the output rounding) for fp64 pre-activations V, G known to within dV, dG."""
+    gl = _gelu64(G)
+    dgelu = (0.5 * (1 + torch.erf(G / math.sqrt(2))) + G * torch.exp(-0.5 * G * G) / math.sqrt(2 * math.pi)).abs()
+    d1 = torch.clamp(dgelu + 0.8 * dG, max=1.13)
+    e_gelu = G.abs() * (2.0 ** -22 + 2.0 ** -18 * torch.erfc(G.abs() / math.sqrt(2))) + 2.0 ** -21 * gl.abs()
+    return V * gl, (gl.abs() * dV + V.abs() * (d1 * dG + e_gelu) + dV * (1.13 * dG + e_gelu) + 2.0 ** -22 * (V * gl).abs())
 
 
 def bound_check(out, ref, bnd, bf16_out=True, residual=None):

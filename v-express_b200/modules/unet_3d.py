@@ -462,7 +462,12 @@ class UNetEngine:
         ops.fold_layernorm), so LayerNorm(x) is never written to HBM.
         The one-kernel variant (ops.gemm_ln: row tile resident in shared memory, statistics computed in the kernel) passes
         its operator tests but is not wired into the engine (it was slower than LayerNorm kernel + GEMM at the 320-wide
-        level when measured)."""
+        level when measured).
+        Validated domain of both modes (tests/test_lnfold_bounds_gpu.py): LayerNorm input rows with |mean| / sigma <=
+        R(K) = 0.8 * 2^12 / (K + 2) (10.2, 5.1, 2.6 at K = 320, 640, 1280) meet the default path's fp64 accuracy bound; the
+        synthetic UNets stay below 0.6.  Beyond R the fold's uncentred accumulation and the hand-over's E[x^2] - mean^2
+        variance (relative rstd error ~ 1.5 (nparts + 2) 2^-24 (mean / sigma)^2, unbounded on near-constant rows) void that
+        guarantee; measured, both stayed at the default path's accuracy up to |mean| / sigma ~ 64."""
         self.ln_fold = os.environ.get("VX_LN_FOLD") == "1"
         # VX_LN_FUSE=1 (experiment, measured: parity green, SLOWER -- stays off): statistics hand-over.  Every LayerNorm
         # input is the output of a Linear (+ residual); that GEMM's epilogue emits per-row partial sums (ops.gemm_rowsums),

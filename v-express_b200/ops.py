@@ -174,7 +174,13 @@ def row_stats(x, eps=1e-5, out=None):
 def fold_layernorm(w, bias, gamma, beta, geglu=False):
     """LayerNorm(x) @ w.T + bias  ==  rstd * (x @ wf.T - mean * colsum) + bf   with
     wf = bf16(w * gamma), colsum = sum_k wf, bf = w @ beta + bias.  w bf16 [N, K]; gamma/beta/bias fp32.
-    geglu=True additionally applies pack_geglu's row order to all three."""
+    geglu=True additionally applies pack_geglu's row order to all three.
+    colsum must be the sum of the ROUNDED wf: then mean * colsum cancels the uncentred part of x @ wf.T exactly and the
+    weight rounding stays a centred 2^-9 r sum |x_k - mean| |gamma_k w_k| (half the default path's LayerNorm output
+    rounding).  What the fold still pays is the uncentred fp32 accumulation, (K + 2) 2^-22 (|mean| / sigma) sum |wf_k| at
+    worst: tests/test_lnfold_bounds_gpu.py holds the fused GEMMs to the default path's accuracy bound for rows with
+    |mean| / sigma <= R(K) = 0.8 * 2^12 / (K + 2) (10.2 at K = 320, 2.6 at K = 1280).  Beyond that, and on near-constant
+    rows, there is no such guarantee; the measured error stayed at the default path's up to |mean| / sigma ~ 64."""
     wf = (w.float() * gamma.float()[None, :]).to(BF16)
     bf = w.float() @ beta.float()
     if bias is not None:
