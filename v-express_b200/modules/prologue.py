@@ -9,9 +9,10 @@ hot path's validated operators plus one gather kernel:
 * AudioProjection (4-layer perceiver resampler, 10 -> 5 tokens per frame): GEMMs, LayerNorm, the exact-softmax attention
   kernel for the 15-key attention, GELU through the GEGLU epilogue with a constant-one value half.
 
-WRITTEN AFTER THE ROUND-1 GPU BUDGET WAS SPENT: not yet run on hardware (tests/test_zz_prologue_gpu.py is skipped unless
-VX_TEST_UNVERIFIED=1).  Oracle + reference-generated golden: oracle/vx_oracle.py (kps_guider_forward,
-audio_projection_forward), tests/golden/prologue_small.pt.
+Checked on the GPU by tests/test_prologue_bounds_gpu.py (every kernel call of a forward against an fp64 reference
+under an elementwise bound, the modules against the fp64 oracle at 512^2 / 768^2 and L up to 1000, the chunking and
+batching invariants) and tests/test_zz_prologue_gpu.py (the reference-generated golden).  Oracle: oracle/vx_oracle.py
+(kps_guider_forward, audio_projection_forward); golden: tests/golden/prologue_small.pt.
 """
 from __future__ import annotations
 

@@ -722,6 +722,10 @@ def im2col3x3(x, NB, H, W, stride=1, silu=False, out=None, pad_lo=1):
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     if out is None:
         out = torch.empty((NB * Ho * Wo, 9 * C), device=x.device, dtype=BF16)
+    # the kernel takes no leading dimensions: rows of x are C apart and rows of out 9 C apart
+    if not x.is_contiguous() or x.shape[0] != NB * H * W or not out.is_contiguous() or out.shape != (NB * Ho * Wo, 9 * C):
+        raise ValueError(f"im2col3x3: x must be a contiguous [{NB * H * W}, C] and out a contiguous [{NB * Ho * Wo}, {9 * C}] "
+                         f"tensor, got x {tuple(x.shape)} strides {x.stride()}, out {tuple(out.shape)} strides {out.stride()}")
     check(_ffi.lib().vx_im2col3x3(ptr(x), c_int(NB), c_int(H), c_int(W), c_int(C), c_int(stride), c_int(int(silu)),
                                   c_int(pad_lo), ptr(out), stream_ptr()), "vx_im2col3x3")
     return out
