@@ -197,12 +197,25 @@ int vx_cfg_overlap_accumulate_n(const void* noise, int n, int f, int hw, int L, 
  * n * 4 * L * hw elements; every sample gets the update a one-sample call would give it. */
 int vx_ddim_step(void* latents, const float* acc, long long n, float sqrt_a, float sqrt_1ma, float sqrt_aprev,
                  float sqrt_1maprev, void* stream);
+/* vx_ddim_step on the k frames listed in `frames` (device int32, each in [0, L)) of latents bf16 / acc fp32, both
+ * (ns, L, hw) with ns = samples x 4 channels, with the same rounding points; those acc entries are set to 0 in the same
+ * pass.  Replaces the per-frame scheduler.step + noise_preds reset of the reference's streaming update
+ * (pipelines/v_express_pipeline.py:566-572) for the wavefront order of VExpressPipeline.stream, where a frame is stepped
+ * as soon as its last window has contributed and frames sit at different steps. */
+int vx_ddim_step_frames(void* latents, float* acc, int ns, int L, int hw, const int* frames, int k, float sqrt_a,
+                        float sqrt_1ma, float sqrt_aprev, float sqrt_1maprev, void* stream);
 
 /* ---- post-processing of the decoded video (SURVEY.md 8f-f3): 3x3x3 median over (t, y, x) with reflect padding
  * (pipelines/utils.py:46-63) and the uint8 frames save_video hands to the encoder (:70-73, truncation of v*255).
  * video [C,T,H,W] fp32 (device); filtered (nullable) same layout; frames (nullable) [T,H,W,C] uint8.
  * Bit-exact vs the reference-generated golden (tests/test_zz_post_gpu.py). */
 int vx_median3d_u8(const float* video, int C, int T, int H, int W, float* filtered, unsigned char* frames, void* stream);
+/* The same filter on a run of frames, for a video decoded chunk by chunk (pipelines/utils.py:46-73 applied piecewise):
+ * buf [C, nbuf, H, W] fp32 holds frames [buf_start, buf_start + nbuf) of a T-frame video and must include every temporal
+ * neighbour of the owned frames [own_start, own_start + own_count) -- one halo frame on each side, time reflected only
+ * at the video's true ends.  frames [own_count, H, W, C] uint8, bit-identical to those frames of vx_median3d_u8. */
+int vx_median3d_range_u8(const float* buf, int C, int nbuf, int buf_start, int own_start, int own_count, int T, int H,
+                         int W, unsigned char* frames, void* stream);
 
 /* ---- nearest-2x upsample folded into the following 3x3 convolution (reference modules/resnet.py:53-90 Upsample3D;
  * diffusers Upsample2D in AutoencoderKL.decode): out = conv3x3(upsample2x(X)) computed as four 2x2 convolutions of X, one per

@@ -392,17 +392,38 @@ __global__ void cfg_overlap_n_kernel(const CfgNArgs p) {
 
 // DDIM v-prediction step on all frames (eta = 0), bf16 rounding after every tensor op like the reference
 // (diffusers DDIMScheduler.step with fp32 scalar coefficients on model-dtype tensors, SURVEY.md B.5).
+__device__ __forceinline__ __nv_bfloat16 ddim_update(float x, float acc, float sa, float sb, float sap, float sbp) {
+  const float v = rbf(acc);   // no-op on one GPU; after the fp32 all-reduce of two bf16 partial sums = their bf16 sum
+  const float x0 = rbf(rbf(sa * x) - rbf(sb * v));
+  const float eps = rbf(rbf(sa * v) + rbf(sb * x));
+  const float dir = rbf(sbp * eps);
+  return __float2bfloat16(rbf(sap * x0) + dir);
+}
+
 __global__ void ddim_step_kernel(__nv_bfloat16* __restrict__ latents, const float* __restrict__ acc, long long n,
                                  float sa, float sb, float sap, float sbp) {
   pdl_enter();
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < n;
+       idx += (long long)gridDim.x * blockDim.x)
+    latents[idx] = ddim_update(__bfloat162float(latents[idx]), acc[idx], sa, sb, sap, sbp);
+}
+
+// The same update on the k frames listed in `frames` of latents / acc (ns, L, hw) -- ns = n samples x 4 channels --
+// zeroing those acc entries for the next step's sums.  The wavefront schedule of VExpressPipeline.stream finalises a
+// frame's step as soon as its last window has contributed, so frames are at different steps and acc is cleared per frame.
+__global__ void ddim_step_frames_kernel(__nv_bfloat16* __restrict__ latents, float* __restrict__ acc, int ns, int L,
+                                        int hw, const int* __restrict__ frames, int k, float sa, float sb, float sap,
+                                        float sbp) {
+  pdl_enter();
+  const long long total = (long long)ns * k * hw;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
-    const float x = __bfloat162float(latents[idx]);
-    const float v = rbf(acc[idx]);   // no-op on one GPU; after the fp32 all-reduce of two bf16 partial sums = their bf16 sum
-    const float x0 = rbf(rbf(sa * x) - rbf(sb * v));
-    const float eps = rbf(rbf(sa * v) + rbf(sb * x));
-    const float dir = rbf(sbp * eps);
-    latents[idx] = __float2bfloat16(rbf(sap * x0) + dir);
+    const int px = (int)(idx % hw);
+    const int j = (int)((idx / hw) % k);
+    const long long sc = idx / ((long long)hw * k);
+    const long long off = (sc * L + frames[j]) * hw + px;
+    latents[off] = ddim_update(__bfloat162float(latents[off]), acc[off], sa, sb, sap, sbp);
+    acc[off] = 0.f;
   }
 }
 
@@ -519,6 +540,19 @@ extern "C" int vx_ddim_step(void* latents, const float* acc, long long n, float 
   if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   launch_k(ddim_step_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (__nv_bfloat16*)latents, acc, n, sqrt_a,
                                                                       sqrt_1ma, sqrt_aprev, sqrt_1maprev);
+  VX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vx_ddim_step_frames(void* latents, float* acc, int ns, int L, int hw, const int* frames, int k, float sqrt_a,
+                                   float sqrt_1ma, float sqrt_aprev, float sqrt_1maprev, void* stream) {
+  VX_REQUIRE(ns >= 1 && L >= 1 && hw >= 1 && k >= 1 && k <= L && frames, "vx_ddim_step_frames: ns=%d L=%d hw=%d k=%d", ns, L,
+             hw, k);
+  const long long total = (long long)ns * k * hw;
+  long long blocks = (total + 255) / 256;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
+  launch_k(ddim_step_frames_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (__nv_bfloat16*)latents, acc, ns,
+           L, hw, frames, k, sqrt_a, sqrt_1ma, sqrt_aprev, sqrt_1maprev);
   VX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

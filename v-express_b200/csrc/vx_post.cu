@@ -4,6 +4,8 @@
 //   tensor per frame and moves every frame device <-> CPU; here one thread owns one output pixel (all channels),
 //   gathers the 27 neighbours through L1 and selects the median with a pruned Batcher odd-even merge network held in
 //   registers (selection, so the result is bit-exact).  Compute-light and HBM-light: 4 B read + 1 B written per value.
+//   The same kernel filters a run of frames of a video decoded chunk by chunk (vx_median3d_range_u8, for
+//   VExpressPipeline.stream): the buffer carries one halo frame on each side and time reflects at the video's ends.
 // Checked on the GPU: the median / uint8 path bit-exact against the oracle and the golden (tests/test_zz_post_gpu.py),
 // im2col3x3 bit-exact as a gather and within an fp64 bound for its SiLU (tests/test_prologue_bounds_gpu.py).
 #include "vx_host.h"
@@ -42,26 +44,29 @@ __device__ __forceinline__ float median27(float (&v)[27]) {
 
 __device__ __forceinline__ int reflect(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * (n - 1) - i : i); }
 
-// video: [C][T][H][W] fp32; filtered (optional): same layout; frames (optional): [T][H][W][C] uint8
-__global__ void __launch_bounds__(256) median3d_kernel(const float* __restrict__ video, int C, int T, int H, int W,
-                                                       float* __restrict__ filtered, unsigned char* __restrict__ frames) {
+// video: [C][nbuf][H][W] fp32 holding frames [buf0, buf0 + nbuf) of a T-frame video; the kernel filters the `nown` frames
+// from own0 on (time reflected at the video's ends 0 and T - 1, not at the buffer's).  filtered (optional): [C][nown][H][W];
+// frames (optional): [nown][H][W][C] uint8.  The whole video is buf0 = own0 = 0, nbuf = nown = T.
+__global__ void __launch_bounds__(256) median3d_kernel(const float* __restrict__ video, int C, int nbuf, int buf0, int own0,
+                                                       int nown, int T, int H, int W, float* __restrict__ filtered,
+                                                       unsigned char* __restrict__ frames) {
   pdl_enter();
-  const long long npix = (long long)T * H * W;
+  const long long npix = (long long)nown * H * W;
   const long long plane = (long long)H * W;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < npix;
        idx += (long long)gridDim.x * blockDim.x) {
     const int x = (int)(idx % W);
     const int y = (int)((idx / W) % H);
-    const int t = (int)(idx / plane);
+    const int t = own0 + (int)(idx / plane);
     int tt[3], yy[3], xx[3];
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
-      tt[d] = reflect(t + d - 1, T);
+      tt[d] = reflect(t + d - 1, T) - buf0;
       yy[d] = reflect(y + d - 1, H);
       xx[d] = reflect(x + d - 1, W);
     }
     for (int c = 0; c < C; ++c) {
-      const float* base = video + (long long)c * T * plane;
+      const float* base = video + (long long)c * nbuf * plane;
       float v[27];
 #pragma unroll
       for (int a = 0; a < 3; ++a)
@@ -70,7 +75,7 @@ __global__ void __launch_bounds__(256) median3d_kernel(const float* __restrict__
 #pragma unroll
           for (int d = 0; d < 3; ++d) v[(a * 3 + b) * 3 + d] = __ldg(base + (long long)tt[a] * plane + (long long)yy[b] * W + xx[d]);
       const float m = median27(v);                 // 14th smallest of 27
-      if (filtered) filtered[(long long)c * T * plane + idx] = m;
+      if (filtered) filtered[(long long)c * nown * plane + idx] = m;
       if (frames) frames[idx * C + c] = (unsigned char)(m * 255.0f);   // truncation, like numpy astype(uint8)
     }
   }
@@ -137,7 +142,28 @@ extern "C" int vx_median3d_u8(const float* video, int C, int T, int H, int W, fl
   const long long npix = (long long)T * H * W;
   long long blocks = (npix + 255) / 256;
   if (blocks > device_sms() * 16) blocks = device_sms() * 16;
-  launch_k(median3d_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, video, C, T, H, W, filtered, frames);
+  launch_k(median3d_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, video, C, T, 0, 0, T, T, H, W, filtered,
+           frames);
+  VX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vx_median3d_range_u8(const float* buf, int C, int nbuf, int buf_start, int own_start, int own_count, int T,
+                                    int H, int W, unsigned char* frames, void* stream) {
+  VX_REQUIRE(C >= 1 && T >= 2 && H >= 2 && W >= 2, "vx_median3d_range_u8: reflect padding needs T, H, W >= 2 (got %d %d %d)",
+             T, H, W);
+  VX_REQUIRE(own_start >= 0 && own_count >= 1 && own_start + own_count <= T && frames,
+             "vx_median3d_range_u8: frames [%d, %d) outside the video of %d", own_start, own_start + own_count, T);
+  // every temporal neighbour of an owned frame (reflected at the video's ends) must be in the buffer
+  const int need_lo = own_start > 0 ? own_start - 1 : 0;
+  const int need_hi = own_start + own_count < T ? own_start + own_count + 1 : T;
+  VX_REQUIRE(buf_start >= 0 && buf_start <= need_lo && buf_start + nbuf >= need_hi && buf_start + nbuf <= T,
+             "vx_median3d_range_u8: buffer [%d, %d) must cover frames [%d, %d)", buf_start, buf_start + nbuf, need_lo, need_hi);
+  const long long npix = (long long)own_count * H * W;
+  long long blocks = (npix + 255) / 256;
+  if (blocks > device_sms() * 16) blocks = device_sms() * 16;
+  launch_k(median3d_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, buf, C, nbuf, buf_start, own_start,
+           own_count, T, H, W, (float*)nullptr, frames);
   VX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -669,6 +669,23 @@ def ddim_step(latents, acc, sqrt_a, sqrt_1ma, sqrt_aprev, sqrt_1maprev):
                                   c_float(sqrt_aprev), c_float(sqrt_1maprev), stream_ptr()), "vx_ddim_step")
 
 
+def ddim_step_frames(latents, acc, frames, sqrt_a, sqrt_1ma, sqrt_aprev, sqrt_1maprev):
+    """ddim_step on the frames listed in ``frames`` (int32 device tensor) of latents bf16 (n,4,L,h,w) / acc fp32
+    (n,4,L,h*w); those acc entries are zeroed in the same pass."""
+    n, c, L = latents.shape[:3]
+    hw = latents[0, 0, 0].numel()
+    if not (latents.dtype == BF16 and acc.dtype == torch.float32 and frames.dtype == torch.int32):
+        raise ValueError(f"ddim_step_frames: latents bf16 / acc fp32 / frames int32, got {latents.dtype} / {acc.dtype} / "
+                         f"{frames.dtype}")
+    if not (latents.is_contiguous() and acc.is_contiguous() and frames.is_contiguous() and acc.numel() == latents.numel()
+            and acc.shape[:3] == latents.shape[:3] and frames.dim() == 1 and 1 <= frames.numel() <= L):
+        raise ValueError(f"ddim_step_frames: latents {tuple(latents.shape)} and acc {tuple(acc.shape)} must be contiguous "
+                         f"(n,4,L,...) of equal size, frames a 1-D list of at most L indices, got {tuple(frames.shape)}")
+    check(_ffi.lib().vx_ddim_step_frames(ptr(latents), ptr(acc), c_int(n * c), c_int(L), c_int(hw), ptr(frames),
+                                         c_int(frames.numel()), c_float(sqrt_a), c_float(sqrt_1ma), c_float(sqrt_aprev),
+                                         c_float(sqrt_1maprev), stream_ptr()), "vx_ddim_step_frames")
+
+
 def softmax_rows(x, out=None):
     """Row softmax of fp32 scores [rows, n] -> bf16 probabilities."""
     _chk_vectors("softmax_rows", 4, x, out)
@@ -712,6 +729,24 @@ def median3d_u8(video, want_filtered=False):
     check(_ffi.lib().vx_median3d_u8(ptr(video), c_int(C), c_int(T), c_int(H), c_int(W), ptr(filt), ptr(frames),
                                     stream_ptr()), "vx_median3d_u8")
     return (frames, filt) if want_filtered else frames
+
+
+def median3d_range_u8(buf, buf_start, own_start, own_count, video_length, out=None):
+    """median3d_u8 of frames [own_start, own_start + own_count) of a ``video_length``-frame video from buf (C,k,H,W) fp32,
+    which holds frames [buf_start, buf_start + k) including one neighbour on each side of the owned run (fewer at the
+    video's ends) -> uint8 (own_count,H,W,C), bit-identical to those frames of median3d_u8 on the whole video."""
+    if not (buf.dtype == torch.float32 and buf.is_contiguous() and buf.dim() == 4):
+        raise ValueError(f"median3d_range_u8: buf must be a contiguous (C,k,H,W) fp32 tensor, got {buf.dtype} "
+                         f"{tuple(buf.shape)}")
+    C, k, H, W = buf.shape
+    if out is None:
+        out = torch.empty((own_count, H, W, C), device=buf.device, dtype=torch.uint8)
+    if out.shape != (own_count, H, W, C) or out.dtype != torch.uint8 or not out.is_contiguous():
+        raise ValueError(f"median3d_range_u8: out must be a contiguous uint8 {(own_count, H, W, C)}, got {tuple(out.shape)}")
+    check(_ffi.lib().vx_median3d_range_u8(ptr(buf), c_int(C), c_int(k), c_int(buf_start), c_int(own_start),
+                                          c_int(own_count), c_int(video_length), c_int(H), c_int(W), ptr(out),
+                                          stream_ptr()), "vx_median3d_range_u8")
+    return out
 
 
 def im2col3x3(x, NB, H, W, stride=1, silu=False, out=None, pad_lo=1):

@@ -4,12 +4,13 @@ results, bit-exact integers).
 Reference: ``uniform`` pipelines/context.py:30-59, ``ordered_halving`` :22-27, ``get_context_scheduler``
 :62-66, ``compute_num_context`` :7-10, ``compute_context_indices`` :13-19.  Host-side integer logic only.
 """
-from typing import Callable, Iterator, List, Optional
+from typing import Callable, Iterator, List, NamedTuple, Optional, Tuple
 
 import numpy as np
 
 __all__ = ["ordered_halving", "uniform", "get_context_scheduler", "compute_num_context",
-           "compute_context_indices", "get_total_steps", "window_table", "overlap_plan"]
+           "compute_context_indices", "get_total_steps", "window_table", "overlap_plan", "Wavefront",
+           "wavefront_schedule"]
 
 
 def compute_num_context(init_video_length: int, context_size: int, context_overlap: int) -> int:
@@ -117,3 +118,56 @@ def overlap_plan(windows, count):
             per_round[r][li] = f
         rounds.append(per_round)
     return rounds
+
+
+class Wavefront(NamedTuple):
+    """Work order of ``wavefront_schedule``; every list but ``order`` is indexed like ``order``."""
+    reach: int                      # R: largest index distance between two windows that share a frame
+    order: List[Tuple[int, int]]    # (window, step) items
+    finalised: List[List[int]]      # frames whose step sum is complete after the item: they get their DDIM update
+    chunks: List[List[Tuple[int, int]]]   # VAE chunks [start, stop) whose frames are all final after the item
+    loads: List[List[int]]          # frames first read by the item (their conditioning must be ready before it)
+    releases: List[List[int]]       # frames no later item reads
+
+
+def wavefront_schedule(windows, num_steps: int, video_length: int, vae_chunk: int) -> Wavefront:
+    """Wavefront order of the ``num_steps`` x ``len(windows)`` window forwards of one video.
+
+    A window at step t reads only its frames' latents after step t - 1, so item (w, t) may run once every window u that
+    shares a frame with w has run step t - 1 and those frames got their DDIM update.  With R the largest |u - w| over such
+    pairs, the key (t R + w, t) orders the items so that
+      * (w, t) comes after (u, t - 1) for every u sharing a frame with w (t R + w >= (t - 1) R + u, ties broken by t);
+      * within one step a frame's contributions arrive in window order, the order ``overlap_plan``'s slot arrays assume,
+        so its step-t sum is complete after its last window and is stepped there -- before any item of step t + 1 reads
+        it and after every item of step t has;
+      * each item appears once.
+    About R (T - 1) + 1 windows are in flight at a time, and the first frames are final after R T (T + 1) / 2 items.
+
+    Chunks are ``vae_chunk`` frames counted from frame 0 (the chunks of ``VExpressPipeline.decode_latents``) and are
+    listed in frame order: a chunk whose frames are final before an earlier chunk's waits for it."""
+    W, L, T = len(windows), video_length, num_steps
+    if W == 0 or T < 1 or vae_chunk < 1:
+        raise ValueError(f"wavefront_schedule: {W} windows, {T} steps, vae_chunk {vae_chunk}")
+    first, last = [W] * L, [-1] * L
+    for wi, win in enumerate(windows):
+        for f in win:
+            first[f], last[f] = min(first[f], wi), max(last[f], wi)
+    if min(last) < 0:
+        raise ValueError(f"wavefront_schedule: frames {[f for f in range(L) if last[f] < 0]} are in no window")
+    # windows sharing a frame lie within [first[f], last[f]] of that frame
+    reach = max(last[f] - first[f] for f in range(L))
+    order = sorted(((w, t) for t in range(T) for w in range(W)), key=lambda it: (it[1] * reach + it[0], it[1]))
+    pos = {it: i for i, it in enumerate(order)}
+    finalised, loads, releases = [[] for _ in order], [[] for _ in order], [[] for _ in order]
+    for f in range(L):
+        loads[pos[(first[f], 0)]].append(f)
+        releases[pos[(last[f], T - 1)]].append(f)
+        for t in range(T):
+            finalised[pos[(last[f], t)]].append(f)
+    chunks = [[] for _ in order]
+    ready = -1
+    for c0 in range(0, L, vae_chunk):
+        c1 = min(c0 + vae_chunk, L)
+        ready = max(ready, max(pos[(last[f], T - 1)] for f in range(c0, c1)))
+        chunks[ready].append((c0, c1))
+    return Wavefront(reach, order, finalised, chunks, loads, releases)

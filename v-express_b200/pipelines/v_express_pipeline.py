@@ -15,7 +15,10 @@ What differs by design (SURVEY.md 0.5, 8e):
   * the VAE decodes all frames of a chunk in one batch;
   * ``num_images_per_prompt`` = n samples of the same conditioning run through ONE UNet forward per window, batched as
     [uncond s0..s(n-1) | cond s0..s(n-1)].  Sample i of an n-sample call is bit-identical to a one-sample call with
-    ``generator[i]`` (the reference accepts the argument but its UNet cannot run it).
+    ``generator[i]`` (the reference accepts the argument but its UNet cannot run it);
+  * ``stream`` runs the same forwards in a wavefront over the windows (``context.wavefront_schedule``) and yields the
+    video chunk by chunk as frames become final, holding kps features only for the windows in flight, so clip length is
+    bounded by ~100 KB of resident state per frame rather than by the features and the video (DESIGN.md 5).
 
 Out of the hot path (SURVEY.md 8f), kept as overridable hooks exactly like the reference methods:
 ``prepare_reference_latent``, ``prepare_kps_feature``, ``prepare_audio_embeddings`` and the ReferenceNet write
@@ -25,18 +28,56 @@ from __future__ import annotations
 
 import math
 import os
-from typing import Callable, List, Optional, Union
+from typing import Callable, Iterator, List, NamedTuple, Optional, Union
 
 import torch
 
 from .. import _ffi, ops
 from ..modules.mutual_self_attention import ReferenceAttentionControl
 from ..modules.unet_3d import UNet3DConditionModel
-from .context import overlap_plan, window_table
+from .context import overlap_plan, wavefront_schedule, window_table
 from .scheduler import ddim_coefficients
 
 BF16 = torch.bfloat16
 _ALLREDUCE_FP32 = os.environ.get("VX_ALLREDUCE_FP32") == "1"     # A/B switch: reduce the fp32 accumulator instead of its bf16 copy
+
+
+class VideoChunk(NamedTuple):
+    """One piece of a streamed video: frames [start, start + k) of every sample, in a fresh pinned host tensor --
+    (n,3,k,H,W) fp32 in [0,1] for ``output="float"``, (n,k,H,W,3) uint8 median-filtered for ``output="uint8"``."""
+    start: int
+    frames: torch.Tensor
+
+
+class _HostCopies:
+    """Device -> pinned host copies on a side stream, each with an event, so the denoising stream never waits for the
+    caller.  The device source is held until its copy has completed.  On a CPU device (the host-side test harness) the
+    copy is a plain clone."""
+
+    def __init__(self, dev):
+        self.cuda = dev.type == "cuda"
+        self.stream = torch.cuda.Stream(dev) if self.cuda else None
+        self.pending = []                  # (key, start, host tensor, device source, event), in frame order
+
+    def push(self, key, start, src):
+        if not self.cuda:
+            self.pending.append((key, start, src.clone(), None, None))
+            return
+        host = torch.empty(tuple(src.shape), dtype=src.dtype, pin_memory=True)
+        self.stream.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(self.stream):
+            host.copy_(src, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(self.stream)
+        self.pending.append((key, start, host, src, ev))
+
+    def ready(self, before_key=None):
+        """Pop (in order) the chunks pushed before ``before_key`` (all when None), waiting for their copies."""
+        while self.pending and (before_key is None or self.pending[0][0] < before_key):
+            _, start, host, _, ev = self.pending.pop(0)
+            if ev is not None:
+                ev.synchronize()
+            yield VideoChunk(start, host)
 
 
 def retrieve_timesteps(scheduler, num_inference_steps=None, device=None, timesteps=None, **kwargs):
@@ -45,6 +86,17 @@ def retrieve_timesteps(scheduler, num_inference_steps=None, device=None, timeste
         raise ValueError("custom timestep schedules are not supported by the DDIM hot path")
     scheduler.set_timesteps(num_inference_steps, device=device, **kwargs)
     return scheduler.timesteps, num_inference_steps
+
+
+def _runs(frames):
+    """Sorted frame indices -> lists of consecutive indices."""
+    out = []
+    for fr in frames:
+        if out and out[-1][-1] + 1 == fr:
+            out[-1].append(fr)
+        else:
+            out.append([fr])
+    return out
 
 
 def partition_windows(num_windows: int, world_size: int, rank: int):
@@ -83,6 +135,14 @@ class _GraphedUNet:
             self.kps = torch.empty_like(kps)
             self.graph = None
         self.kps.copy_(kps)
+
+    def kps_ring(self, rows, channels):
+        """The static kps buffer as a ring of ``rows`` channels-last rows that the caller fills in place between
+        replays (``stream``); an existing buffer of that shape is reused, so its captured graph stays valid."""
+        if self.kps is None or self.kps.shape != (rows, channels):
+            self.set_kps(torch.zeros((rows, channels), device=self.frames.device, dtype=BF16))
+        self.kps_token = self.kps
+        return self.kps
 
     def __call__(self, temb):
         if self.temb is None:
@@ -215,6 +275,21 @@ class VExpressPipeline:
         if do_classifier_free_guidance:
             kps_feature = torch.cat([torch.zeros_like(kps_feature), kps_feature], dim=0)
         return kps_feature
+
+    def prepare_kps_feature_frames(self, kps_images, start, stop, height, width):
+        """Frames [start, stop) of ``prepare_kps_feature``'s conditional half, (1, 320, stop - start, h, w) on the device,
+        for ``stream``, which holds only the frames its windows in flight read.  Converts only the images of the 16-frame
+        chunks (aligned at multiples of 16, as ``prepare_kps_feature`` runs them) that hold those frames and runs the
+        guider on those chunks, so the result is bit-identical to the slice of the whole-video features."""
+        if self.v_kps_guider is None:
+            raise NotImplementedError("prologue hook: pass a VKpsGuider (vexpress_b200.modules.VKpsGuider or the "
+                                      "reference's) or override prepare_kps_feature_frames with precomputed features")
+        c0, c1 = start // 16 * 16, -(-stop // 16) * 16
+        images = kps_images[:, :, c0:c1] if torch.is_tensor(kps_images) else kps_images[c0:c1]
+        x = self._condition_images_to_tensor(images, height, width)
+        feats = [self.v_kps_guider(x[:, :, i:i + 16].to(device=self.device, dtype=self.dtype))
+                 for i in range(0, x.shape[2], 16)]
+        return torch.cat(feats, dim=2)[:, :, start - c0:stop - c0]
 
     @staticmethod
     def audio_frame_windows(audio_embeddings, video_length, num_pad_audio_frames):
@@ -384,6 +459,133 @@ class VExpressPipeline:
         return latents
 
     @torch.no_grad()
+    def denoise_stream(self, latents, kps_images, audio_embeddings, timesteps, guidance_scale, context_frames,
+                       context_overlap, context_schedule="uniform", output="float") -> Iterator[VideoChunk]:
+        """``denoise`` + decode as a generator of ``VideoChunk``s in frame order, in device memory that does not grow with
+        the video beyond latents, acc, audio tokens and the count table.  The same forwards on the same inputs as
+        ``denoise``, in the wavefront order of ``context.wavefront_schedule``: a frame gets its DDIM update as soon as its
+        last window of the step has contributed (``ops.ddim_step_frames``), and a VAE chunk is decoded as soon as its
+        frames are final, so the frames and final latents are bit-identical to ``denoise`` + ``decode_to_device``.
+
+        kps features exist only for the frames of the windows in flight: a ring of frame slots that is the captured
+        graph's static kps buffer, filled through ``prepare_kps_feature_frames(kps_images, ...)`` before a frame's first
+        read and recycled after its last.  Uncond rows all read slot 0, a zero frame.  latents (n,4,L,h,w) bf16 device
+        (updated in place); audio_embeddings (b,L,T,768).  ``output="uint8"`` yields ``ops.median3d_range_u8`` of each
+        chunk, which waits for the first frame of the next one."""
+        if output not in ("float", "uint8"):
+            raise ValueError(f"output must be 'float' or 'uint8', got {output!r}")
+        unet: UNet3DConditionModel = self.denoising_unet
+        eng = unet.engine()
+        dev = latents.device
+        n, _, L, h, w = latents.shape
+        hw = h * w
+        H, W = h * self.vae_scale_factor, w * self.vae_scale_factor
+        do_cfg = guidance_scale > 1.0
+        b = 2 if do_cfg else 1
+        windows, count = window_table(L, context_frames, context_overlap, context_schedule)
+        f = len(windows[0])
+        if any(len(wn) != f for wn in windows):
+            raise ValueError(f"stream needs windows of one size, the {context_schedule!r} schedule gave "
+                             f"{sorted(set(len(wn) for wn in windows))}")
+        plan = overlap_plan(windows, count)
+        sched = wavefront_schedule(windows, len(timesteps), L, self.vae_chunk)
+        # kps ring slots, planned on the host: a frame holds its slot from its first read to its last; slot 0 = zeros
+        slot_of, free, nslots, fills = {}, [], 0, []
+        kps_idx, fin = {}, {}
+        for i, (wi, t) in enumerate(sched.order):
+            fills.append([])
+            for fr in sched.loads[i]:
+                if not free:
+                    nslots += 1
+                    free.append(nslots)
+                slot_of[fr] = free.pop()
+                fills[i].append(fr)
+            if t == 0:
+                rows = [0] * (n * f) if do_cfg else []
+                kps_idx[wi] = torch.tensor(rows + [slot_of[fr] for fr in windows[wi]] * n, dtype=torch.int32,
+                                           device=dev)
+                fin[wi] = torch.tensor(sched.finalised[i], dtype=torch.int32, device=dev) if sched.finalised[i] else None
+            for fr in sched.releases[i]:
+                free.append(slot_of[fr])
+        count_dev = torch.from_numpy(count).to(device=dev, dtype=torch.int32)
+        audio = audio_embeddings.to(device=dev, dtype=BF16, non_blocking=True)
+        T = audio.shape[2]
+        acc = torch.zeros((n, 4, L, hw), device=dev, dtype=torch.float32)
+        win_long = [torch.tensor(wn, device=dev, dtype=torch.long) for wn in windows]
+        plan_dev = [[torch.from_numpy(r).to(dev) for r in rounds] for rounds in plan]
+        for name in eng.order:
+            eng._bank_kv(name, unet.get_submodule(name))
+        key = (b, n, f, h, w, T, bool(self.use_cuda_graph), eng.graph_signature())
+        g = self._graphs.get(key)
+        if g is None:
+            for k_old in [k for k in self._graphs if k[:5] == key[:5] and k != key]:
+                del self._graphs[k_old]
+            g = self._graphs[key] = _GraphedUNet(eng, b, f, h, w, T, audio.shape[-1], self.use_cuda_graph, n)
+        tembs = [eng.time_embedding(int(t)) for t in timesteps]
+        coeffs = [ddim_coefficients(self.scheduler, int(t)) for t in timesteps]
+        ring = None
+        copies = _HostCopies(dev)
+        tail = None                     # uint8: decoded frames [tail_start, ...) = halo frame + the chunk not yet filtered
+        tail_start = own_start = 0
+
+        def filtered(buf, buf_start, start, stop):
+            u8 = torch.empty((n, stop - start, H, W, 3), device=dev, dtype=torch.uint8)
+            for s in range(n):
+                ops.median3d_range_u8(buf[s], buf_start, start, stop - start, L, out=u8[s])
+            return u8
+
+        cur_key = None
+        for i, (wi, t) in enumerate(sched.order):
+            item_key = t * sched.reach + wi
+            if item_key != cur_key:
+                if cur_key is not None:
+                    yield from copies.ready(before_key=cur_key)    # every item of the key after theirs is enqueued
+                cur_key = item_key
+            for run in _runs(fills[i]):
+                feat = self.prepare_kps_feature_frames(kps_images, run[0], run[-1] + 1, H, W)
+                rows = feat[0].to(device=dev, dtype=BF16).permute(1, 2, 3, 0).reshape(len(run), hw, -1)
+                if ring is None:
+                    ring = g.kps_ring((nslots + 1) * hw, rows.shape[-1]).view(nslots + 1, hw, -1)
+                    ring[0].zero_()
+                for j, fr in enumerate(run):
+                    ring[slot_of[fr]].copy_(rows[j])
+            x = latents[:, :, win_long[wi]].transpose(1, 2)                     # (n,f,4,h,w)
+            g.frames.view(b, n, f, 4, h, w).copy_(x)
+            g.enc.view(b, n, f, T, -1).copy_(audio[:, win_long[wi]].unsqueeze(1))
+            g.kps_idx.copy_(kps_idx[wi])
+            noise = g(tembs[t])
+            for slots in plan_dev[wi]:
+                if n == 1:
+                    ops.cfg_overlap_accumulate(noise, f, hw, L, do_cfg, slots, count_dev, float(guidance_scale), acc[0])
+                else:
+                    ops.cfg_overlap_accumulate_n(noise, n, f, hw, L, do_cfg, slots, count_dev, float(guidance_scale), acc)
+            if fin[wi] is not None:
+                ops.ddim_step_frames(latents, acc, fin[wi], *coeffs[t])
+            for c0, c1 in sched.chunks[i]:
+                vid = torch.empty((n, 3, c1 - c0, H, W), device=dev, dtype=torch.float32)
+                for s in range(n):
+                    self.decode_latents(latents, range(c0, c1), out=vid[s], sample=s)
+                if output == "float":
+                    copies.push(item_key, c0, vid)
+                    continue
+                if tail is not None:
+                    copies.push(item_key, own_start, filtered(torch.cat([tail, vid[:, :, :1]], 2), tail_start, own_start, c0))
+                    tail, tail_start = torch.cat([tail[:, :, -1:], vid], 2), c0 - 1
+                else:
+                    tail = vid
+                own_start = c0
+        if tail is not None:
+            copies.push(cur_key, own_start, filtered(tail, tail_start, own_start, L))
+        yield from copies.ready()
+
+    @staticmethod
+    def _check_sampling_args(eta, num_images_per_prompt):
+        if eta != 0.0:
+            raise ValueError("the DDIM hot path is deterministic (eta = 0), like the reference CLI")
+        if not isinstance(num_images_per_prompt, int) or num_images_per_prompt < 1:
+            raise ValueError(f"num_images_per_prompt must be a positive integer, got {num_images_per_prompt!r}")
+
+    @torch.no_grad()
     def mean_overlap(self, reference_image, kps_images, audio_waveform, width, height, video_length,
                      num_inference_steps, guidance_scale, strength=1., num_images_per_prompt=1, eta: float = 0.0,
                      generator: Optional[Union[torch.Generator, List[torch.Generator]]] = None,
@@ -392,10 +594,7 @@ class VExpressPipeline:
                      context_schedule="uniform", context_frames=24, context_overlap=4, reference_attention_weight=1.,
                      audio_attention_weight=1., num_pad_audio_frames=2, do_multi_devices_inference=False,
                      save_gpu_memory=False, **kwargs):
-        if eta != 0.0:
-            raise ValueError("the DDIM hot path is deterministic (eta = 0), like the reference CLI")
-        if not isinstance(num_images_per_prompt, int) or num_images_per_prompt < 1:
-            raise ValueError(f"num_images_per_prompt must be a positive integer, got {num_images_per_prompt!r}")
+        self._check_sampling_args(eta, num_images_per_prompt)
         device = self.device
         do_cfg = guidance_scale > 1.0
         batch_size = 1
@@ -491,3 +690,57 @@ class VExpressPipeline:
             context_overlap=context_overlap, reference_attention_weight=reference_attention_weight,
             audio_attention_weight=audio_attention_weight, num_pad_audio_frames=num_pad_audio_frames,
             do_multi_devices_inference=do_multi_devices_inference, save_gpu_memory=save_gpu_memory, **kwargs)
+
+    def stream(self, reference_image, kps_images, audio_waveform, width, height, video_length, num_inference_steps,
+               guidance_scale, strength=1., num_images_per_prompt=1, eta: float = 0.0, generator=None,
+               output_type: Optional[str] = "tensor", return_dict: bool = True, context_schedule="uniform",
+               context_frames=24, context_overlap=4, reference_attention_weight=1., audio_attention_weight=1.,
+               num_pad_audio_frames=2, do_multi_devices_inference=False, save_gpu_memory=False, output="float",
+               **kwargs) -> Iterator[VideoChunk]:
+        """``__call__`` as a generator of ``VideoChunk(start, frames)`` for videos of any length: chunks of
+        ``vae_chunk`` frames in frame order covering [0, video_length) once, each handed out as soon as its frames are
+        final, with the device holding the per-frame state of the whole video (latents, accumulator, audio tokens:
+        about 100 KB per frame and sample at 512x512) but kps features only for the windows in flight
+        (``denoise_stream``).  ``output="float"``: (n,3,k,H,W) fp32 frames equal to the matching frames of ``__call__``;
+        ``output="uint8"``: (n,k,H,W,3) median-filtered uint8 frames, the frames ``save_video`` writes.  Runs on one
+        GPU.  Arguments are checked when called; the work starts with the first ``next``."""
+        self._check_sampling_args(eta, num_images_per_prompt)
+        if output not in ("float", "uint8"):
+            raise ValueError(f"output must be 'float' or 'uint8', got {output!r}")
+        if torch.distributed.is_available() and torch.distributed.is_initialized() \
+                and torch.distributed.get_world_size() > 1:
+            raise ValueError("stream() runs on one GPU: multi-GPU streaming is not supported "
+                             f"(world size {torch.distributed.get_world_size()})")
+        return self._stream(reference_image, kps_images, audio_waveform, width, height, video_length,
+                            num_inference_steps, guidance_scale, strength, num_images_per_prompt, generator,
+                            context_schedule, context_frames, context_overlap, reference_attention_weight,
+                            audio_attention_weight, num_pad_audio_frames, output)
+
+    @torch.no_grad()
+    def _stream(self, reference_image, kps_images, audio_waveform, width, height, video_length, num_inference_steps,
+                guidance_scale, strength, num_images_per_prompt, generator, context_schedule, context_frames,
+                context_overlap, reference_attention_weight, audio_attention_weight, num_pad_audio_frames, output):
+        device = self.device
+        do_cfg = guidance_scale > 1.0
+        timesteps, num_inference_steps = retrieve_timesteps(self.scheduler, num_inference_steps, device, None)
+        timesteps, num_inference_steps = self.get_timesteps(num_inference_steps, strength, device)
+        writer = ReferenceAttentionControl(self.reference_net, do_classifier_free_guidance=do_cfg, mode="write",
+                                           batch_size=1, fusion_blocks="full")
+        reader = ReferenceAttentionControl(self.denoising_unet, do_classifier_free_guidance=do_cfg, mode="read",
+                                           batch_size=1, fusion_blocks="full",
+                                           reference_attention_weight=reference_attention_weight,
+                                           audio_attention_weight=audio_attention_weight)
+        reference_image_latents = self.prepare_reference_latent(reference_image, height, width)
+        audio_embeddings = self.prepare_audio_embeddings(audio_waveform, video_length, num_pad_audio_frames, do_cfg)
+        self.run_reference_net(reference_image_latents, writer)
+        reader.update(getattr(self.reference_net, "writer_view", writer), do_cfg, dtype=self.dtype)
+        latents = self.prepare_latents(num_images_per_prompt, self.denoising_unet.in_channels, width, height,
+                                       video_length, self.dtype, torch.device("cpu"), generator)
+        latents = latents.to(device=device, dtype=BF16, non_blocking=True)
+        try:
+            yield from self.denoise_stream(latents, kps_images, audio_embeddings, timesteps, guidance_scale,
+                                           context_frames, context_overlap, context_schedule, output)
+        finally:
+            reader.clear()
+            if isinstance(getattr(writer, "unet", None), torch.nn.Module) and hasattr(writer, "clear"):
+                writer.clear()
