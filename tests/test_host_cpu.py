@@ -186,12 +186,13 @@ def test_refnet_layout_and_writer_pairing_cpu():
     assert all(len(b.bank) == 0 for b in blocks)
 
 
-def _cpu_engine(cls, model):
-    """Engine object with the packed weights on the CPU (no kernels are called by packing)."""
+def _cpu_engine(cls, model, device="cpu"):
+    """Engine object with the packed weights on the CPU (no kernels are called by packing); device="meta" packs shapes
+    only, for a model built on the meta device."""
     import torch
     from vexpress_b200.modules import unet_3d
     eng = object.__new__(cls)
-    eng.model, eng.dev = model, torch.device("cpu")
+    eng.model, eng.dev = model, torch.device(device)
     c = model.config
     eng.boc = tuple(c["block_out_channels"])
     eng.heads, eng.groups, eng.eps, eng.cross = model.heads, c["norm_num_groups"], float(c["norm_eps"]), c["cross_attention_dim"]
