@@ -576,7 +576,9 @@ def test_ops_wrappers_reject_misaligned_views():
 # ------------------------------------------------------------------------------------------------------------ GPU cases
 # (NB, HW, C1, C2, eps, silu) of every GroupNorm the UNet and ReferenceNet issue at configs[0] (512 x 512, 2 x 4 frames)
 # and at 768 x 768 (2 x 16 frames), recorded with the shape-checking fake ops of tests/test_host_cpu.py; the VAE decoder's
-# (one frame per launch: mid block and up blocks of 512 / 512 / 256 / 128 channels, eps 1e-6) follow its structure.
+# (mid block and up blocks of 512 / 512 / 256 / 128 channels, eps 1e-6) follow its structure at one frame per launch.  The
+# decoder runs 16 frames per launch (the pipeline's vae_chunk), which changes the dispatch's S: those shapes, and the tail
+# chunks of 1..15 frames, are checked frame by frame in tests/test_vae_chunk_bounds_gpu.py.
 GN_UNET = [
     (1, 64, 1280, 0, 1e-05, True), (1, 64, 1280, 1280, 1e-05, True), (1, 256, 640, 0, 1e-05, True),
     (1, 256, 1280, 0, 1e-05, True), (1, 256, 1280, 640, 1e-05, True), (1, 256, 1280, 1280, 1e-05, True),

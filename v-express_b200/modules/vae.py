@@ -244,8 +244,14 @@ class VaeDecoderEngine:
         self.boc = tuple(model.config["block_out_channels"])
         self.layers = model.config["layers_per_block"]
         self.W: Dict[str, torch.Tensor] = {}
+        self._pack({k: v for k, v in nn.Module.state_dict(model).items()
+                    if not (k.startswith("encoder.") or k.startswith("quant_conv."))})
+
+    def _pack(self, msd):
+        """The decoder parameters of ``msd`` (``post_quant_conv.*``, ``decoder.*``) in the kernels' layouts, into ``self.W``
+        on ``self.dev``.  Host-side tensor operations only (no kernel is launched), so it also packs on the CPU or the meta
+        device."""
         dev = self.dev
-        msd = {k: v for k, v in nn.Module.state_dict(model).items() if not (k.startswith("encoder.") or k.startswith("quant_conv."))}
         self.W.update(ops.f32_arena({k: v for k, v in msd.items() if k.endswith(".bias") or v.dim() == 1}, dev))
         for k, v in msd.items():
             v = v.detach()
