@@ -197,6 +197,12 @@ int vx_cfg_overlap_accumulate_n(const void* noise, int n, int f, int hw, int L, 
  * n * 4 * L * hw elements; every sample gets the update a one-sample call would give it. */
 int vx_ddim_step(void* latents, const float* acc, long long n, float sqrt_a, float sqrt_1ma, float sqrt_aprev,
                  float sqrt_1maprev, void* stream);
+/* Stochastic DDIM (eta > 0, diffusers DDIMScheduler.step with variance noise): vx_ddim_step with c_dir =
+ * sqrt(1 - a_prev - sigma^2) in place of sqrt(1 - a_prev), then latents = bf16(prev + bf16(sigma * noise)).  noise is
+ * fp32 with the layout of latents (n contiguous elements): the draw of the model dtype widened, so no rounding precedes
+ * the multiply. */
+int vx_ddim_step_eta(void* latents, const float* acc, const float* noise, long long n, float sqrt_a, float sqrt_1ma,
+                     float sqrt_aprev, float c_dir, float sigma, void* stream);
 /* vx_ddim_step on the k frames listed in `frames` (device int32, each in [0, L)) of latents bf16 / acc fp32, both
  * (ns, L, hw) with ns = samples x 4 channels, with the same rounding points; those acc entries are set to 0 in the same
  * pass.  Replaces the per-frame scheduler.step + noise_preds reset of the reference's streaming update

@@ -408,6 +408,20 @@ __global__ void ddim_step_kernel(__nv_bfloat16* __restrict__ latents, const floa
     latents[idx] = ddim_update(__bfloat162float(latents[idx]), acc[idx], sa, sb, sap, sbp);
 }
 
+// Stochastic DDIM (eta > 0): the same update with c_dir = sqrt(1 - a_prev - sigma^2) in place of sqrt(1 - a_prev),
+// then diffusers' `prev_sample + std_dev_t * variance_noise` on model-dtype tensors: bf16(sigma * noise), then the bf16
+// add.  noise is the fp32 image of the draw (exact for bf16 / fp16 / fp32 draws), laid out like latents.
+__global__ void ddim_step_eta_kernel(__nv_bfloat16* __restrict__ latents, const float* __restrict__ acc,
+                                     const float* __restrict__ noise, long long n, float sa, float sb, float sap,
+                                     float c_dir, float sigma) {
+  pdl_enter();
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < n;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const float prev = __bfloat162float(ddim_update(__bfloat162float(latents[idx]), acc[idx], sa, sb, sap, c_dir));
+    latents[idx] = __float2bfloat16(prev + rbf(sigma * noise[idx]));
+  }
+}
+
 // The same update on the k frames listed in `frames` of latents / acc (ns, L, hw) -- ns = n samples x 4 channels --
 // zeroing those acc entries for the next step's sums.  The wavefront schedule of VExpressPipeline.stream finalises a
 // frame's step as soon as its last window has contributed, so frames are at different steps and acc is cleared per frame.
@@ -540,6 +554,17 @@ extern "C" int vx_ddim_step(void* latents, const float* acc, long long n, float 
   if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   launch_k(ddim_step_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (__nv_bfloat16*)latents, acc, n, sqrt_a,
                                                                       sqrt_1ma, sqrt_aprev, sqrt_1maprev);
+  VX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vx_ddim_step_eta(void* latents, const float* acc, const float* noise, long long n, float sqrt_a,
+                                float sqrt_1ma, float sqrt_aprev, float c_dir, float sigma, void* stream) {
+  VX_REQUIRE(n >= 1 && latents && acc && noise, "vx_ddim_step_eta: n=%lld", n);
+  long long blocks = (n + 255) / 256;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
+  launch_k(ddim_step_eta_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (__nv_bfloat16*)latents, acc,
+           noise, n, sqrt_a, sqrt_1ma, sqrt_aprev, c_dir, sigma);
   VX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

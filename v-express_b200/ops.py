@@ -669,6 +669,21 @@ def ddim_step(latents, acc, sqrt_a, sqrt_1ma, sqrt_aprev, sqrt_1maprev):
                                   c_float(sqrt_aprev), c_float(sqrt_1maprev), stream_ptr()), "vx_ddim_step")
 
 
+def ddim_step_eta(latents, acc, noise, sqrt_a, sqrt_1ma, sqrt_aprev, c_dir, sigma):
+    """Stochastic DDIM step on all elements of latents bf16 (n,4,L,...): ``ddim_step`` with c_dir for sqrt(1-a_prev),
+    plus bf16(sigma * noise); noise fp32 with the layout of latents (``scheduler.ddim_coefficients_eta``)."""
+    if not (latents.dtype == BF16 and acc.dtype == torch.float32 and noise.dtype == torch.float32):
+        raise ValueError(f"ddim_step_eta: latents bf16 / acc fp32 / noise fp32, got {latents.dtype} / {acc.dtype} / "
+                         f"{noise.dtype}")
+    if not (latents.is_contiguous() and acc.is_contiguous() and noise.is_contiguous()
+            and acc.numel() == latents.numel() == noise.numel() and latents.device == acc.device == noise.device):
+        raise ValueError(f"ddim_step_eta: latents {tuple(latents.shape)}, acc {tuple(acc.shape)} and noise "
+                         f"{tuple(noise.shape)} must be contiguous tensors of equal size on one device")
+    check(_ffi.lib().vx_ddim_step_eta(ptr(latents), ptr(acc), ptr(noise), c_ll(latents.numel()), c_float(sqrt_a),
+                                      c_float(sqrt_1ma), c_float(sqrt_aprev), c_float(c_dir), c_float(sigma),
+                                      stream_ptr()), "vx_ddim_step_eta")
+
+
 def ddim_step_frames(latents, acc, frames, sqrt_a, sqrt_1ma, sqrt_aprev, sqrt_1maprev):
     """ddim_step on the frames listed in ``frames`` (int32 device tensor) of latents bf16 (n,4,L,h,w) / acc fp32
     (n,4,L,h*w); those acc entries are zeroed in the same pass."""

@@ -9,7 +9,7 @@ from typing import Callable, Iterator, List, NamedTuple, Optional, Tuple
 import numpy as np
 
 __all__ = ["ordered_halving", "uniform", "get_context_scheduler", "compute_num_context",
-           "compute_context_indices", "get_total_steps", "window_table", "overlap_plan", "Wavefront",
+           "compute_context_indices", "get_total_steps", "window_table", "overlap_plan", "step_frame_ids", "Wavefront",
            "wavefront_schedule"]
 
 
@@ -77,25 +77,24 @@ def window_table(video_length: int, context_frames: int, context_overlap: int, s
     return windows, count
 
 
-def overlap_plan(windows, count):
-    """Which window slots end up in a frame's noise prediction, for window lists that may repeat a frame inside one
-    (reflected) window.  Integer replay of the reference's streaming bookkeeping (pipelines/v_express_pipeline.py
-    :528-529,552-572): per window ``context_counter[context] += 1`` is a NON-accumulating index-put (a repeated frame
-    counts once), the Python loop then walks the slots in order, starts a frame's sum at its first slot
-    (``noise_preds[f] is None``), adds every further slot, and each time ``context_counter[f] == num_frame_context[f]``
-    holds it hands the current sum to ``scheduler.step`` and resets it -- so a frame repeated inside its LAST window is
-    stepped more than once from the same input latents and the last write wins (index-put on the host tensor).
+def _streaming_replay(windows, count):
+    """Integer replay of the reference's streaming bookkeeping (pipelines/v_express_pipeline.py :528-529,552-572): per
+    window ``context_counter[context] += 1`` is a NON-accumulating index-put (a repeated frame counts once), the Python
+    loop then walks the slots in order, starts a frame's sum at its first slot (``noise_preds[f] is None``), adds every
+    further slot, and each time ``context_counter[f] == num_frame_context[f]`` holds it hands the current sum to
+    ``scheduler.step`` and resets it.
 
-    Returns ``rounds[w]`` = list of int32 arrays of len(windows[w]): entry = frame index if that slot's prediction is
-    accumulated into the frame's final sum, -1 if the reference discards it; every array holds each frame at most
-    once, and the arrays of one window are in the reference's summation order."""
+    Returns (final, steps): ``final[f]`` = the (window, slot) list of the sum whose step lands last in frame f, and
+    ``steps[w]`` = the ``step_frame_ids`` window w hands to ``scheduler.step``, in order, repeats included."""
     L = len(count)
     counter = [0] * L
     pending = [None] * L
     final = {}
+    steps = []
     for wi, win in enumerate(windows):
         for f in set(win):
             counter[f] += 1
+        ids = []
         for li, f in enumerate(win):
             if pending[f] is None:
                 pending[f] = []
@@ -103,6 +102,27 @@ def overlap_plan(windows, count):
             if counter[f] == int(count[f]):
                 final[f] = pending[f]
                 pending[f] = None
+                ids.append(f)
+        steps.append(ids)
+    return final, steps
+
+
+def step_frame_ids(windows, count):
+    """Per window, the frames the reference hands to ``scheduler.step`` (its ``step_frame_ids``), in order, a frame
+    repeated inside a reflected window once per time it is stepped; the step's ``latents[:, :, ids] = ...`` write
+    keeps the last.  A frame is stepped only inside its last window, so every frame appears in exactly one list."""
+    return _streaming_replay(windows, count)[1]
+
+
+def overlap_plan(windows, count):
+    """Which window slots end up in a frame's noise prediction, for window lists that may repeat a frame inside one
+    (reflected) window, from the replay of ``_streaming_replay``: a frame repeated inside its LAST window is stepped
+    more than once from the same input latents and the last write wins (index-put on the host tensor).
+
+    Returns ``rounds[w]`` = list of int32 arrays of len(windows[w]): entry = frame index if that slot's prediction is
+    accumulated into the frame's final sum, -1 if the reference discards it; every array holds each frame at most
+    once, and the arrays of one window are in the reference's summation order."""
+    final, _ = _streaming_replay(windows, count)
     keep = set(slot for slots in final.values() for slot in slots)
     rounds = []
     for wi, win in enumerate(windows):

@@ -1,7 +1,7 @@
 """DDIM scheduler restated for the hot path (diffusers 0.29.2 ``DDIMScheduler`` with the reference's
 configuration inference_v2.yaml:23-33: scaled-linear betas, zero-terminal-SNR rescale, v-prediction, trailing
-timestep spacing, eta = 0; SURVEY.md Appendix B.5).  Host-side scalar tables only: the tensor update itself is the
-fused ``vx_ddim_step`` kernel."""
+timestep spacing; SURVEY.md Appendix B.5).  Host-side scalar tables only: the tensor update itself is the fused
+``vx_ddim_step`` kernel, or ``vx_ddim_step_eta`` for stochastic DDIM (eta > 0)."""
 from types import SimpleNamespace
 
 import numpy as np
@@ -59,3 +59,29 @@ def ddim_coefficients(scheduler, timestep: int):
     a_p = (scheduler.alphas_cumprod[prev] if prev >= 0 else scheduler.final_alpha_cumprod).float().cpu()
     b_t = 1 - a_t
     return float(a_t ** 0.5), float(b_t ** 0.5), float(a_p ** 0.5), float((1 - a_p) ** 0.5)
+
+
+def ddim_coefficients_eta(scheduler, timestep: int, eta: float):
+    """(sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), c_dir, sigma) for the stochastic step (``vx_ddim_step_eta``), from the
+    fp32 0-d tensor arithmetic of diffusers' ``step`` / ``_get_variance``:
+
+        variance = (1-a_prev)/(1-a_t) * (1 - a_t/a_prev);  sigma = eta * variance ** 0.5
+        c_dir    = (1 - a_prev - sigma ** 2) ** 0.5
+
+    so each scalar equals the library's bit for bit -- with one exception: where that radicand rounds below zero
+    (eta = 1 at a_t = 0, the first trailing step of a zero-terminal-SNR schedule: sigma ** 2 rounds one ulp above
+    1 - a_prev at 25 steps), the library's 0-d ``** 0.5`` is NaN and the whole video with it; c_dir is 0 here, the exact
+    value.  At eta = 0, sigma = 0 and c_dir = sqrt(1 - a_prev): the first four entries and c_dir are ``ddim_coefficients``."""
+    if not 0.0 <= eta <= 1.0:
+        raise ValueError(f"eta must lie in [0, 1], got {eta!r}")
+    cfg = scheduler.config
+    if getattr(cfg, "prediction_type", "v_prediction") != "v_prediction":
+        raise ValueError("only v_prediction is supported")
+    prev = int(timestep) - cfg.num_train_timesteps // scheduler.num_inference_steps
+    a_t = scheduler.alphas_cumprod[int(timestep)].float().cpu()
+    a_p = (scheduler.alphas_cumprod[prev] if prev >= 0 else scheduler.final_alpha_cumprod).float().cpu()
+    b_t, b_p = 1 - a_t, 1 - a_p
+    variance = (b_p / b_t) * (1 - a_t / a_p)
+    sigma = eta * variance ** 0.5
+    c_dir = (1 - a_p - sigma ** 2).clamp_min(0) ** 0.5
+    return float(a_t ** 0.5), float(b_t ** 0.5), float(a_p ** 0.5), float(c_dir), float(sigma)

@@ -16,6 +16,8 @@ What differs by design (SURVEY.md 0.5, 8e):
   * ``num_images_per_prompt`` = n samples of the same conditioning run through ONE UNet forward per window, batched as
     [uncond s0..s(n-1) | cond s0..s(n-1)].  Sample i of an n-sample call is bit-identical to a one-sample call with
     ``generator[i]`` (the reference accepts the argument but its UNet cannot run it);
+  * ``eta > 0`` draws the reference's per-window variance noise on the host (or, generator None, on the device) while
+    the step's window forwards run, and adds it in the step's one DDIM launch (``_StepNoise``, DESIGN.md 5);
   * ``stream`` runs the same forwards in a wavefront over the windows (``context.wavefront_schedule``) and yields the
     video chunk by chunk as frames become final, holding kps features only for the windows in flight, so clip length is
     bounded by ~100 KB of resident state per frame rather than by the features and the video (DESIGN.md 5).
@@ -35,8 +37,8 @@ import torch
 from .. import _ffi, ops
 from ..modules.mutual_self_attention import ReferenceAttentionControl
 from ..modules.unet_3d import UNet3DConditionModel
-from .context import overlap_plan, wavefront_schedule, window_table
-from .scheduler import ddim_coefficients
+from .context import overlap_plan, step_frame_ids, wavefront_schedule, window_table
+from .scheduler import ddim_coefficients, ddim_coefficients_eta
 
 BF16 = torch.bfloat16
 _ALLREDUCE_FP32 = os.environ.get("VX_ALLREDUCE_FP32") == "1"     # A/B switch: reduce the fp32 accumulator instead of its bf16 copy
@@ -78,6 +80,86 @@ class _HostCopies:
             if ev is not None:
                 ev.synchronize()
             yield VideoChunk(start, host)
+
+
+def _draw_device(generator, device):
+    """Where diffusers' ``randn_tensor(..., generator, device)`` draws: on the host for a CPU generator (then moved), on
+    ``device`` for a generator there or for None (torch's default generator of that device)."""
+    device = torch.device(device)
+    if generator is None:
+        return device
+    gen_type = (generator[0] if isinstance(generator, list) else generator).device.type
+    if gen_type != device.type and gen_type == "cpu":
+        return torch.device("cpu")
+    if gen_type != device.type:
+        raise ValueError(f"Cannot generate a {device} tensor from a generator of type {gen_type}.")
+    return device
+
+
+def _randn(shape, generator, device, dtype):
+    """diffusers.utils.torch_utils.randn_tensor (0.29.2) without the final move: the draw on ``_draw_device``.  A list
+    of generators draws sample i as a (1, ...) tensor from ``generator[i]``; a list of one is the generator itself."""
+    rand_device = _draw_device(generator, device)
+    if isinstance(generator, list) and len(generator) == 1:
+        generator = generator[0]
+    if isinstance(generator, list):
+        one = (1,) + tuple(shape[1:])
+        return torch.cat([torch.randn(one, generator=g, device=rand_device, dtype=dtype) for g in generator])
+    return torch.randn(shape, generator=generator, device=rand_device, dtype=dtype)
+
+
+class _StepNoise:
+    """The variance noise of one stochastic DDIM step (eta > 0), as the reference draws it.
+
+    Per step the reference calls ``scheduler.step`` once per window, in window order, on the frames the window finalises
+    (``context.step_frame_ids``, a frame repeated in a reflected window once per occurrence), and diffusers' step draws
+    ``randn_tensor(model_output.shape, generator, device=model_output.device, dtype=model_output.dtype)`` -- (n,4,k,h,w)
+    in the model dtype -- then ``latents[:, :, ids] = ...`` keeps a repeated frame's LAST occurrence.  ``draw`` replays
+    those draws and scatters the element each frame keeps into ``buf``, (n,4,L,hw) fp32 on the device (fp32 holds bf16,
+    fp16 and fp32 draws exactly).  Host draws (a CPU generator, the reference CLI's case) land in a fresh pinned buffer
+    from torch's caching host allocator -- a block is not handed out again before its copy has run -- and reach ``buf``
+    by one non-blocking copy, so the step never waits on the device; device draws (generator None) scatter in place.
+    ``draws=False`` (ranks other than 0) skips the draws: ``buf`` then comes from rank 0's broadcast."""
+
+    def __init__(self, windows, count, shape, dtype, generator, device, draws=True):
+        n, c, L, h, w = shape
+        if isinstance(generator, list) and len(generator) != n:
+            raise ValueError(f"You have passed a list of generators of length {len(generator)}, but requested an "
+                             f"effective batch size of {n}. Make sure the batch size matches the length of the "
+                             f"generators.")
+        self.shape, self.dtype, self.generator, self.draws = (n, c, L, h, w), dtype, generator, draws
+        self.rand_device = _draw_device(generator, device)
+        self.buf = torch.empty((n, c, L, h * w), device=device, dtype=torch.float32)
+        self.plan = []                     # per drawing window: (k, frame slice or index tensor, draw slots or None)
+        covered = 0
+        for ids in step_frame_ids(windows, count):
+            if not ids:
+                continue                   # a window that finalises nothing makes no step call
+            last = {fr: j for j, fr in enumerate(ids)}
+            frames = sorted(last)
+            covered += len(frames)
+            if ids == list(range(ids[0], ids[0] + len(ids))):
+                self.plan.append((len(ids), slice(frames[0], frames[-1] + 1), None))     # consecutive, no repeats
+            else:
+                self.plan.append((len(ids), torch.tensor(frames, device=self.rand_device),
+                                  torch.tensor([last[fr] for fr in frames], device=self.rand_device)))
+        if covered != L:
+            raise ValueError(f"the context windows step {covered} of {L} frames")
+
+    def draw(self):
+        if not self.draws:
+            return
+        n, c, L, h, w = self.shape
+        staged = self.rand_device != self.buf.device
+        dst = torch.empty((n, c, L, h * w), dtype=torch.float32, pin_memory=True) if staged else self.buf
+        for k, frames, slots in self.plan:
+            x = _randn((n, c, k, h, w), self.generator, self.rand_device, self.dtype).view(n, c, k, h * w)
+            if slots is None:
+                dst[:, :, frames].copy_(x)
+            else:
+                dst[:, :, frames] = x[:, :, slots].to(torch.float32)
+        if staged:
+            self.buf.copy_(dst, non_blocking=True)
 
 
 def retrieve_timesteps(scheduler, num_inference_steps=None, device=None, timesteps=None, **kwargs):
@@ -337,11 +419,7 @@ class VExpressPipeline:
                              f"effective batch size of {batch_size}. Make sure the batch size matches the length of "
                              f"the generators.")
         if latents is None:
-            if isinstance(generator, list):
-                latents = torch.cat([torch.randn((1,) + shape[1:], generator=g, device="cpu", dtype=dtype)
-                                     for g in generator])
-            else:
-                latents = torch.randn(shape, generator=generator, device="cpu", dtype=dtype)
+            latents = _randn(shape, generator, "cpu", dtype)
         return latents * self.scheduler.init_noise_sigma
 
     def get_timesteps(self, num_inference_steps, strength, device):
@@ -371,12 +449,17 @@ class VExpressPipeline:
     # ------------------------------------------------------------------ the hot loop
     @torch.no_grad()
     def denoise(self, latents, kps_feature, audio_embeddings, timesteps, guidance_scale, context_frames,
-                context_overlap, context_schedule="uniform", distributed=False, callback=None, callback_steps=1):
+                context_overlap, context_schedule="uniform", distributed=False, callback=None, callback_steps=1,
+                eta=0.0, generator=None):
         """latents (n,4,L,h,w) bf16 device (updated in place and returned); kps_feature (b,C0,L,h,w) device;
         audio_embeddings (b,L,T,768) device.  Steps x windows with overlap averaging, CFG and DDIM
         (reference :486-500,514-589).  The n samples share the conditioning and step together: one UNet forward per window
         on the batch [uncond s0..s(n-1) | cond s0..s(n-1)] whose frames all gather their kps rows from the one resident
-        copy, one CFG / overlap launch per window, one DDIM launch per step."""
+        copy, one CFG / overlap launch per window, one DDIM launch per step.
+
+        eta > 0 (stochastic DDIM): each step draws the reference's variance noise from ``generator`` (``_StepNoise``)
+        while the step's window forwards run on the GPU, and applies it in the step's one ``vx_ddim_step_eta`` launch.
+        Under ``distributed`` rank 0 draws and broadcasts the step's noise.  eta = 0 draws nothing."""
         unet: UNet3DConditionModel = self.denoising_unet
         eng = unet.engine()
         dev = latents.device
@@ -416,6 +499,7 @@ class VExpressPipeline:
         for name in eng.order:
             eng._bank_kv(name, unet.get_submodule(name))
         graphs = self._graphs
+        step_noise = _StepNoise(windows, count, latents.shape, self.dtype, generator, dev, rank == 0) if eta > 0 else None
         for i, t in enumerate(timesteps):
             temb = eng.time_embedding(int(t))
             acc.zero_()
@@ -443,6 +527,8 @@ class VExpressPipeline:
                     else:
                         ops.cfg_overlap_accumulate_n(noise, n, f, hw, L, do_cfg, slots, count_dev, float(guidance_scale),
                                                      acc)
+            if step_noise is not None:
+                step_noise.draw()                       # host work while the window forwards above run on the GPU
             if world > 1:
                 # every frame has at most two non-zero bf16 contributions across the ranks (its windows live on one rank
                 # or on two neighbours), so the bf16 sum is the reference's own bf16 add -- half the bytes of fp32
@@ -452,8 +538,13 @@ class VExpressPipeline:
                     acc_x.copy_(acc)
                     torch.distributed.all_reduce(acc_x, op=torch.distributed.ReduceOp.SUM)
                     acc.copy_(acc_x)
-            sa, sb, sap, sbp = ddim_coefficients(self.scheduler, int(t))
-            ops.ddim_step(latents, acc, sa, sb, sap, sbp)                   # elementwise over all n samples
+                if step_noise is not None:
+                    torch.distributed.broadcast(step_noise.buf, src=0)      # rank 0's draw is THE noise
+            if step_noise is None:
+                sa, sb, sap, sbp = ddim_coefficients(self.scheduler, int(t))
+                ops.ddim_step(latents, acc, sa, sb, sap, sbp)               # elementwise over all n samples
+            else:
+                ops.ddim_step_eta(latents, acc, step_noise.buf, *ddim_coefficients_eta(self.scheduler, int(t), eta))
             if callback is not None and i % callback_steps == 0:
                 callback(i, t, latents)
         return latents
@@ -579,9 +670,17 @@ class VExpressPipeline:
         yield from copies.ready()
 
     @staticmethod
-    def _check_sampling_args(eta, num_images_per_prompt):
-        if eta != 0.0:
-            raise ValueError("the DDIM hot path is deterministic (eta = 0), like the reference CLI")
+    def _check_sampling_args(eta, num_images_per_prompt, streaming=False):
+        if streaming and eta != 0.0:
+            raise ValueError("stream() runs deterministic DDIM only (eta = 0): its wavefront interleaves the steps, so "
+                             "it cannot draw the step noise in the order __call__ draws it; use __call__ for eta > 0")
+        try:
+            in_range = 0.0 <= float(eta) <= 1.0                  # False for NaN
+        except (TypeError, ValueError):
+            in_range = False
+        if not in_range:
+            # zero-terminal-SNR makes a_t = 0 at the first trailing step, where eta > 1 takes the root of a negative number
+            raise ValueError(f"eta must be a number in [0, 1], got {eta!r}")
         if not isinstance(num_images_per_prompt, int) or num_images_per_prompt < 1:
             raise ValueError(f"num_images_per_prompt must be a positive integer, got {num_images_per_prompt!r}")
 
@@ -624,7 +723,8 @@ class VExpressPipeline:
             torch.distributed.broadcast(latents, src=0)
         try:
             latents = self.denoise(latents, kps_feature, audio_embeddings, timesteps, guidance_scale, context_frames,
-                                   context_overlap, context_schedule, distributed, callback, callback_steps)
+                                   context_overlap, context_schedule, distributed, callback, callback_steps,
+                                   eta=float(eta), generator=generator)
         finally:
             reader.clear()
             if isinstance(getattr(writer, "unet", None), torch.nn.Module) and hasattr(writer, "clear"):
@@ -703,8 +803,9 @@ class VExpressPipeline:
         about 100 KB per frame and sample at 512x512) but kps features only for the windows in flight
         (``denoise_stream``).  ``output="float"``: (n,3,k,H,W) fp32 frames equal to the matching frames of ``__call__``;
         ``output="uint8"``: (n,k,H,W,3) median-filtered uint8 frames, the frames ``save_video`` writes.  Runs on one
-        GPU.  Arguments are checked when called; the work starts with the first ``next``."""
-        self._check_sampling_args(eta, num_images_per_prompt)
+        GPU, deterministic DDIM only (eta = 0).  Arguments are checked when called; the work starts with the first
+        ``next``."""
+        self._check_sampling_args(eta, num_images_per_prompt, streaming=True)
         if output not in ("float", "uint8"):
             raise ValueError(f"output must be 'float' or 'uint8', got {output!r}")
         if torch.distributed.is_available() and torch.distributed.is_initialized() \
