@@ -210,6 +210,21 @@ int vx_ddim_step_eta(void* latents, const float* acc, const float* noise, long l
  * as soon as its last window has contributed and frames sit at different steps. */
 int vx_ddim_step_frames(void* latents, float* acc, int ns, int L, int hw, const int* frames, int k, float sqrt_a,
                         float sqrt_1ma, float sqrt_aprev, float sqrt_1maprev, void* stream);
+/* DPM-Solver++ multistep step (diffusers DPMSolverMultistepScheduler: dpmsolver++, midpoint, v-prediction) on n
+ * contiguous elements of latents bf16, in place of the per-window scheduler.step of pipelines/v_express_pipeline.py:566-572.
+ * With v = bf16(acc) and x the latent: m0 = bf16(bf16(alpha_s x) - bf16(sigma_s v)) (the x0 prediction);
+ * order 1: latents = bf16(fp32(ratio x) - bf16(c0 m0));
+ * order 2: D1 = bf16(inv_r0 bf16(m0 - x0_prev)), latents = bf16(fp32(ratio x) - bf16(c0 m0) - bf16(c0h D1)), in fp32
+ * left to right.  x0_prev (bf16, the layout of latents) holds the previous step's m0 and receives this step's; order 1
+ * does not read it.  Scalars from scheduler.dpm_coefficients. */
+int vx_dpmpp_step(void* latents, const float* acc, void* x0_prev, long long n, float alpha_s, float sigma_s, float ratio,
+                  float c0, float inv_r0, float c0h, int order, void* stream);
+/* vx_dpmpp_step on the k frames listed in `frames` (device int32, each in [0, L)) of latents bf16 / acc fp32 / x0_prev
+ * bf16, all (ns, L, hw), zeroing those acc entries in the same pass: the per-frame scheduler.step + noise_preds reset of
+ * pipelines/v_express_pipeline.py:566-572 for the wavefront order of VExpressPipeline.stream (as vx_ddim_step_frames). */
+int vx_dpmpp_step_frames(void* latents, float* acc, void* x0_prev, int ns, int L, int hw, const int* frames, int k,
+                         float alpha_s, float sigma_s, float ratio, float c0, float inv_r0, float c0h, int order,
+                         void* stream);
 
 /* ---- post-processing of the decoded video (SURVEY.md 8f-f3): 3x3x3 median over (t, y, x) with reflect padding
  * (pipelines/utils.py:46-63) and the uint8 frames save_video hands to the encoder (:70-73, truncation of v*255).

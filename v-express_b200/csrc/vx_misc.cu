@@ -441,6 +441,54 @@ __global__ void ddim_step_frames_kernel(__nv_bfloat16* __restrict__ latents, flo
   }
 }
 
+// DPM-Solver++ (diffusers DPMSolverMultistepScheduler, algorithm_type "dpmsolver++", solver_type "midpoint",
+// v-prediction) with the rounding points of the library's eager arithmetic on bf16 CUDA tensors: convert_model_output
+// runs on the bf16 sample, so the x0 prediction m0 and the history are bf16; step then upcasts the sample to fp32, so
+// ratio * x stays fp32 while every fp32-scalar x bf16-tensor product rounds to bf16; prev_sample is cast back to bf16.
+// The fp32 products and differences are spelled with _rn intrinsics so that no FMA contraction changes them.
+struct DpmCoeffs {
+  float alpha_s, sigma_s, ratio, c0, inv_r0, c0h;  // c0 = alpha_t (e^-h - 1), c0h = 0.5 c0; inv_r0 / c0h: order 2 only
+  int order;
+};
+
+__device__ __forceinline__ void dpmpp_update(__nv_bfloat16* lat, float acc, __nv_bfloat16* hist, const DpmCoeffs& c) {
+  const float x = __bfloat162float(*lat);
+  const float m0 = rbf(rbf(c.alpha_s * x) - rbf(c.sigma_s * rbf(acc)));
+  float xt = __fsub_rn(__fmul_rn(c.ratio, x), rbf(c.c0 * m0));
+  if (c.order == 2) {
+    const float d1 = rbf(c.inv_r0 * rbf(m0 - __bfloat162float(*hist)));
+    xt = __fsub_rn(xt, rbf(c.c0h * d1));
+  }
+  *hist = __float2bfloat16(m0);
+  *lat = __float2bfloat16(xt);
+}
+
+__global__ void dpmpp_step_kernel(__nv_bfloat16* __restrict__ latents, const float* __restrict__ acc,
+                                  __nv_bfloat16* __restrict__ x0_prev, long long n, DpmCoeffs c) {
+  pdl_enter();
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < n;
+       idx += (long long)gridDim.x * blockDim.x)
+    dpmpp_update(latents + idx, acc[idx], x0_prev + idx, c);
+}
+
+// The same update on the k frames listed in `frames`, zeroing those acc entries (the wavefront of
+// VExpressPipeline.stream, as ddim_step_frames_kernel).
+__global__ void dpmpp_step_frames_kernel(__nv_bfloat16* __restrict__ latents, float* __restrict__ acc,
+                                         __nv_bfloat16* __restrict__ x0_prev, int ns, int L, int hw,
+                                         const int* __restrict__ frames, int k, DpmCoeffs c) {
+  pdl_enter();
+  const long long total = (long long)ns * k * hw;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int px = (int)(idx % hw);
+    const int j = (int)((idx / hw) % k);
+    const long long sc = idx / ((long long)hw * k);
+    const long long off = (sc * L + frames[j]) * hw + px;
+    dpmpp_update(latents + off, acc[off], x0_prev + off, c);
+    acc[off] = 0.f;
+  }
+}
+
 }  // namespace vx
 
 using namespace vx;
@@ -578,6 +626,33 @@ extern "C" int vx_ddim_step_frames(void* latents, float* acc, int ns, int L, int
   if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   launch_k(ddim_step_frames_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (__nv_bfloat16*)latents, acc, ns,
            L, hw, frames, k, sqrt_a, sqrt_1ma, sqrt_aprev, sqrt_1maprev);
+  VX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vx_dpmpp_step(void* latents, const float* acc, void* x0_prev, long long n, float alpha_s, float sigma_s,
+                             float ratio, float c0, float inv_r0, float c0h, int order, void* stream) {
+  VX_REQUIRE(n >= 1 && latents && acc && x0_prev && (order == 1 || order == 2), "vx_dpmpp_step: n=%lld order=%d", n,
+             order);
+  long long blocks = (n + 255) / 256;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
+  launch_k(dpmpp_step_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (__nv_bfloat16*)latents, acc,
+           (__nv_bfloat16*)x0_prev, n, DpmCoeffs{alpha_s, sigma_s, ratio, c0, inv_r0, c0h, order});
+  VX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vx_dpmpp_step_frames(void* latents, float* acc, void* x0_prev, int ns, int L, int hw, const int* frames,
+                                    int k, float alpha_s, float sigma_s, float ratio, float c0, float inv_r0, float c0h,
+                                    int order, void* stream) {
+  VX_REQUIRE(ns >= 1 && L >= 1 && hw >= 1 && k >= 1 && k <= L && frames && latents && acc && x0_prev &&
+                 (order == 1 || order == 2),
+             "vx_dpmpp_step_frames: ns=%d L=%d hw=%d k=%d order=%d", ns, L, hw, k, order);
+  const long long total = (long long)ns * k * hw;
+  long long blocks = (total + 255) / 256;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
+  launch_k(dpmpp_step_frames_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (__nv_bfloat16*)latents,
+           acc, (__nv_bfloat16*)x0_prev, ns, L, hw, frames, k, DpmCoeffs{alpha_s, sigma_s, ratio, c0, inv_r0, c0h, order});
   VX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

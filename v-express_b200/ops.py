@@ -701,6 +701,49 @@ def ddim_step_frames(latents, acc, frames, sqrt_a, sqrt_1ma, sqrt_aprev, sqrt_1m
                                          c_float(sqrt_1maprev), stream_ptr()), "vx_ddim_step_frames")
 
 
+def _dpm_args(alpha_s, sigma_s, ratio, c0, inv_r0, c0h, order):
+    if order not in (1, 2):
+        raise ValueError(f"dpmpp_step: order must be 1 or 2, got {order!r}")
+    return (c_float(alpha_s), c_float(sigma_s), c_float(ratio), c_float(c0), c_float(inv_r0), c_float(c0h), c_int(order))
+
+
+def dpmpp_step(latents, acc, x0_prev, alpha_s, sigma_s, ratio, c0, inv_r0, c0h, order):
+    """DPM-Solver++ step on all elements of latents bf16 (n,4,L,...): acc fp32 is the averaged model output, x0_prev bf16
+    the previous step's x0 prediction (read at order 2), overwritten with this step's; scalars from
+    ``scheduler.dpm_coefficients``."""
+    if not (latents.dtype == BF16 and acc.dtype == torch.float32 and x0_prev.dtype == BF16):
+        raise ValueError(f"dpmpp_step: latents bf16 / acc fp32 / x0_prev bf16, got {latents.dtype} / {acc.dtype} / "
+                         f"{x0_prev.dtype}")
+    if not (latents.is_contiguous() and acc.is_contiguous() and x0_prev.is_contiguous()
+            and acc.numel() == latents.numel() == x0_prev.numel() and latents.device == acc.device == x0_prev.device):
+        raise ValueError(f"dpmpp_step: latents {tuple(latents.shape)}, acc {tuple(acc.shape)} and x0_prev "
+                         f"{tuple(x0_prev.shape)} must be contiguous tensors of equal size on one device")
+    check(_ffi.lib().vx_dpmpp_step(ptr(latents), ptr(acc), ptr(x0_prev), c_ll(latents.numel()),
+                                   *_dpm_args(alpha_s, sigma_s, ratio, c0, inv_r0, c0h, order), stream_ptr()),
+          "vx_dpmpp_step")
+
+
+def dpmpp_step_frames(latents, acc, x0_prev, frames, alpha_s, sigma_s, ratio, c0, inv_r0, c0h, order):
+    """dpmpp_step on the frames listed in ``frames`` (int32 device tensor) of latents bf16 (n,4,L,h,w) / acc fp32 /
+    x0_prev bf16 (n,4,L,h*w); those acc entries are zeroed in the same pass."""
+    n, c, L = latents.shape[:3]
+    hw = latents[0, 0, 0].numel()
+    if not (latents.dtype == BF16 and acc.dtype == torch.float32 and x0_prev.dtype == BF16
+            and frames.dtype == torch.int32):
+        raise ValueError(f"dpmpp_step_frames: latents bf16 / acc fp32 / x0_prev bf16 / frames int32, got {latents.dtype} "
+                         f"/ {acc.dtype} / {x0_prev.dtype} / {frames.dtype}")
+    if not (latents.is_contiguous() and acc.is_contiguous() and x0_prev.is_contiguous() and frames.is_contiguous()
+            and acc.numel() == latents.numel() == x0_prev.numel() and acc.shape[:3] == latents.shape[:3]
+            and x0_prev.shape[:3] == latents.shape[:3] and frames.dim() == 1 and 1 <= frames.numel() <= L):
+        raise ValueError(f"dpmpp_step_frames: latents {tuple(latents.shape)}, acc {tuple(acc.shape)} and x0_prev "
+                         f"{tuple(x0_prev.shape)} must be contiguous (n,4,L,...) of equal size, frames a 1-D list of at "
+                         f"most L indices, got {tuple(frames.shape)}")
+    check(_ffi.lib().vx_dpmpp_step_frames(ptr(latents), ptr(acc), ptr(x0_prev), c_int(n * c), c_int(L), c_int(hw),
+                                          ptr(frames), c_int(frames.numel()),
+                                          *_dpm_args(alpha_s, sigma_s, ratio, c0, inv_r0, c0h, order), stream_ptr()),
+          "vx_dpmpp_step_frames")
+
+
 def softmax_rows(x, out=None):
     """Row softmax of fp32 scores [rows, n] -> bf16 probabilities."""
     _chk_vectors("softmax_rows", 4, x, out)

@@ -18,6 +18,9 @@ What differs by design (SURVEY.md 0.5, 8e):
     ``generator[i]`` (the reference accepts the argument but its UNet cannot run it);
   * ``eta > 0`` draws the reference's per-window variance noise on the host (or, generator None, on the device) while
     the step's window forwards run, and adds it in the step's one DDIM launch (``_StepNoise``, DESIGN.md 5);
+  * a ``DPMSolverMultistepScheduler`` (ours or diffusers') runs DPM-Solver++(2M): one ``vx_dpmpp_step`` per step with
+    a per-frame history of x0 predictions, which at several windows departs from the reference's ill-defined per-window
+    scheduler state (``_LatentUpdate``, DESIGN.md 5);
   * ``stream`` runs the same forwards in a wavefront over the windows (``context.wavefront_schedule``) and yields the
     video chunk by chunk as frames become final, holding kps features only for the windows in flight, so clip length is
     bounded by ~100 KB of resident state per frame rather than by the features and the video (DESIGN.md 5).
@@ -38,7 +41,7 @@ from .. import _ffi, ops
 from ..modules.mutual_self_attention import ReferenceAttentionControl
 from ..modules.unet_3d import UNet3DConditionModel
 from .context import overlap_plan, step_frame_ids, wavefront_schedule, window_table
-from .scheduler import ddim_coefficients, ddim_coefficients_eta
+from .scheduler import ddim_coefficients, ddim_coefficients_eta, dpm_coefficients, dpm_scheduler
 
 BF16 = torch.bfloat16
 _ALLREDUCE_FP32 = os.environ.get("VX_ALLREDUCE_FP32") == "1"     # A/B switch: reduce the fp32 accumulator instead of its bf16 copy
@@ -160,6 +163,60 @@ class _StepNoise:
                 dst[:, :, frames] = x[:, :, slots].to(torch.float32)
         if staged:
             self.buf.copy_(dst, non_blocking=True)
+
+
+class _LatentUpdate:
+    """The per-step latent update of one call, chosen from the scheduler here and nowhere else.  DDIM (every scheduler
+    but DPM-Solver++): ``vx_ddim_step``, ``vx_ddim_step_eta`` when given the step's noise, ``vx_ddim_step_frames``.
+    DPM-Solver++ (``scheduler.dpm_scheduler``): ``vx_dpmpp_step`` / ``vx_dpmpp_step_frames`` with a (n,4,L,hw) bf16
+    history holding each frame's previous x0 prediction; it takes no eta and draws nothing.  ``i`` is the position in
+    the call's ``timesteps``, which may be a ``strength`` slice of the scheduler's schedule."""
+
+    def __init__(self, scheduler, timesteps, latents):
+        self.scheduler, self.timesteps = scheduler, [int(t) for t in timesteps]
+        self.dpm = dpm_scheduler(scheduler)
+        self.coeffs = {}
+        if self.dpm is None:
+            return
+        full = self.dpm.timesteps.tolist()
+        self.offset = len(full) - len(self.timesteps)
+        if self.offset < 0 or full[self.offset:] != self.timesteps:
+            raise ValueError("the timesteps are not a tail of the DPM-Solver++ schedule set_timesteps made")
+        n, c, L = latents.shape[:3]
+        self.history = torch.empty((n, c, L, latents[0, 0, 0].numel()), device=latents.device, dtype=BF16)
+
+    @property
+    def draws_noise(self):
+        """Whether a step takes variance noise at eta > 0 (stochastic DDIM)."""
+        return self.dpm is None
+
+    def _coeffs(self, i, eta=None):
+        key = (i, eta)
+        if key not in self.coeffs:
+            if self.dpm is not None:
+                self.coeffs[key] = dpm_coefficients(self.dpm, self.offset + i, first=i == 0)
+            elif eta is None:
+                self.coeffs[key] = ddim_coefficients(self.scheduler, self.timesteps[i])
+            else:
+                self.coeffs[key] = ddim_coefficients_eta(self.scheduler, self.timesteps[i], eta)
+        return self.coeffs[key]
+
+    def step(self, i, latents, acc, noise=None, eta=0.0):
+        """Step ``i`` on every frame of latents (n,4,L,h,w) from acc (n,4,L,hw); ``noise`` (DDIM at eta > 0) the step's
+        variance noise, fp32 with the layout of acc."""
+        if self.dpm is not None:
+            ops.dpmpp_step(latents, acc, self.history, *self._coeffs(i))
+        elif noise is None:
+            ops.ddim_step(latents, acc, *self._coeffs(i))               # elementwise over all n samples
+        else:
+            ops.ddim_step_eta(latents, acc, noise, *self._coeffs(i, eta))
+
+    def step_frames(self, i, latents, acc, frames):
+        """Step ``i`` on the frames listed in ``frames`` (int32 device tensor), zeroing their acc entries."""
+        if self.dpm is not None:
+            ops.dpmpp_step_frames(latents, acc, self.history, frames, *self._coeffs(i))
+        else:
+            ops.ddim_step_frames(latents, acc, frames, *self._coeffs(i))
 
 
 def retrieve_timesteps(scheduler, num_inference_steps=None, device=None, timesteps=None, **kwargs):
@@ -459,7 +516,8 @@ class VExpressPipeline:
 
         eta > 0 (stochastic DDIM): each step draws the reference's variance noise from ``generator`` (``_StepNoise``)
         while the step's window forwards run on the GPU, and applies it in the step's one ``vx_ddim_step_eta`` launch.
-        Under ``distributed`` rank 0 draws and broadcasts the step's noise.  eta = 0 draws nothing."""
+        Under ``distributed`` rank 0 draws and broadcasts the step's noise.  eta = 0 draws nothing.  With a DPM-Solver++
+        scheduler the step's launch is ``vx_dpmpp_step`` and eta is ignored (``_LatentUpdate``)."""
         unet: UNet3DConditionModel = self.denoising_unet
         eng = unet.engine()
         dev = latents.device
@@ -499,7 +557,9 @@ class VExpressPipeline:
         for name in eng.order:
             eng._bank_kv(name, unet.get_submodule(name))
         graphs = self._graphs
-        step_noise = _StepNoise(windows, count, latents.shape, self.dtype, generator, dev, rank == 0) if eta > 0 else None
+        update = _LatentUpdate(self.scheduler, timesteps, latents)
+        step_noise = _StepNoise(windows, count, latents.shape, self.dtype, generator, dev, rank == 0) \
+            if eta > 0 and update.draws_noise else None
         for i, t in enumerate(timesteps):
             temb = eng.time_embedding(int(t))
             acc.zero_()
@@ -540,11 +600,7 @@ class VExpressPipeline:
                     acc.copy_(acc_x)
                 if step_noise is not None:
                     torch.distributed.broadcast(step_noise.buf, src=0)      # rank 0's draw is THE noise
-            if step_noise is None:
-                sa, sb, sap, sbp = ddim_coefficients(self.scheduler, int(t))
-                ops.ddim_step(latents, acc, sa, sb, sap, sbp)               # elementwise over all n samples
-            else:
-                ops.ddim_step_eta(latents, acc, step_noise.buf, *ddim_coefficients_eta(self.scheduler, int(t), eta))
+            update.step(i, latents, acc, None if step_noise is None else step_noise.buf, eta)
             if callback is not None and i % callback_steps == 0:
                 callback(i, t, latents)
         return latents
@@ -613,7 +669,7 @@ class VExpressPipeline:
                 del self._graphs[k_old]
             g = self._graphs[key] = _GraphedUNet(eng, b, f, h, w, T, audio.shape[-1], self.use_cuda_graph, n)
         tembs = [eng.time_embedding(int(t)) for t in timesteps]
-        coeffs = [ddim_coefficients(self.scheduler, int(t)) for t in timesteps]
+        update = _LatentUpdate(self.scheduler, timesteps, latents)
         ring = None
         copies = _HostCopies(dev)
         tail = None                     # uint8: decoded frames [tail_start, ...) = halo frame + the chunk not yet filtered
@@ -651,7 +707,7 @@ class VExpressPipeline:
                 else:
                     ops.cfg_overlap_accumulate_n(noise, n, f, hw, L, do_cfg, slots, count_dev, float(guidance_scale), acc)
             if fin[wi] is not None:
-                ops.ddim_step_frames(latents, acc, fin[wi], *coeffs[t])
+                update.step_frames(t, latents, acc, fin[wi])
             for c0, c1 in sched.chunks[i]:
                 vid = torch.empty((n, 3, c1 - c0, H, W), device=dev, dtype=torch.float32)
                 for s in range(n):
